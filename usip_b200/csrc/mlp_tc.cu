@@ -6,35 +6,47 @@
 //     D += a_lo*w_hi + a_hi*w_lo + a_hi*w_hi        (dropped term a_lo*w_lo ~ 2^-22 relative)
 // which keeps fp32-level accuracy (the 1e-4 parity bar) at 1/3 of the TF32 tensor rate.
 //
-// Persistent CTA (one per SM) of two warpgroups (256 threads) on 128-row x BN-column output tiles; warpgroup g owns rows
-// 64g..64g+63 of the tile and accumulates them in registers with wgmma.mma_async (m64 x BN x k8, operands in shared memory).
-// Per 32-float K chunk:
-//   * every thread loads its share of the X chunk (float4, one chunk ahead in registers), applies the folded BN affine +
-//     ReLU, splits hi/lo and writes the 128B-swizzled A tiles with st.shared;
-//   * thread 0 fetches the pre-split, pre-swizzled weight tile with one bulk-TMA copy (cp.async.bulk) two chunks ahead;
-//   * each warpgroup issues 12 wgmma (4 k-steps x 3 products) and keeps them in flight while the next A tile is written.
-// Three shared-memory stages.  A stage is rewritten only after both warpgroups retired the wgmma group that read it:
-// wgmma.wait_group 1 in each warpgroup, then the CTA barrier that ends the chunk.
-// Epilogue per tile: accumulators (+addend, +bias) -> XOR-swizzled [128 x BN] fp32 tile in the idle stage memory -> eight
-// warps on 32-row x 32-column chunks: coalesced Y stores, BN statistic partials, per-group max/min (+arg).
+// Persistent CTA (one per SM) of two consumer warpgroups and one producer warpgroup.  A CTA keeps one BN-wide column tile and
+// walks its row tiles base, base + stride, ...  Each warpgroup accumulates 64-row x BN tiles in registers with
+// wgmma.mma_async (m64 x BN x k8): it takes every other 64-row tile of the CTA's sequence, or, with COMBINE (group-128
+// max/min), one 64-row half of every 128-row tile.
+//   * A comes from registers.  Every thread loads the raw fp32 values of its own fragment straight from global memory one
+//     K chunk ahead (crossing into the warpgroup's next tile), applies the folded BN affine + ReLU and splits hi/lo.  Two
+//     fragment buffers alternate; a buffer is rewritten only after wgmma.wait_group retired the chunk that read it.
+//   * B (the pre-split, pre-swizzled weight tile of one K chunk) streams through one shared-memory ring that both
+//     warpgroups read, since they run through the same column tile's chunks.  The producer lane refills a stage with one
+//     bulk-TMA copy once both warpgroups arrived on its empty barrier; the full barrier counts the copy's bytes.  When the
+//     whole K panel fits in the ring (KC <= stages) it is loaded once and never recycled.
+//   * Nothing in the main loop couples the two warpgroups, so one runs its tensor work while the other is in its epilogue.
+// Epilogue per warpgroup tile: accumulators (+addend, +bias) -> the warpgroup's XOR-swizzled [64 x BN] fp32 staging tile
+// -> four warps on 32-row x 32-column chunks: coalesced Y stores, BN statistic partials, per-group max/min (+arg).
 //
-// Operand tiles are K-major, SWIZZLE_128B: row r (128 B = 32 tf32) at r*128, 16-byte chunk c stored at chunk (c ^ (r & 7));
+// K order inside a 32-float chunk: the wgmma fragment holds k = l%4 and l%4 + 4 of each k-step, so logical position p of
+// k-step s reads physical column 8*(p%4) + 2s + p/4.  Thread quad position t then owns physical columns 8t..8t+7 of both of
+// its rows (two float4 each), and a quad reads one contiguous 128-byte row segment.  In 16-byte-chunk terms the logical
+// column 4c + j holds physical column 8j + c; the weight pack applies the same map, and a dot product ignores K order.
+//
+// B tiles are K-major, SWIZZLE_128B: row r (128 B = 32 tf32) at r*128, 16-byte chunk c stored at chunk (c ^ (r & 7));
 // 8-row groups 1024 B apart.  One K chunk = 32 floats = 4 wgmma k-steps of 8.
 #include "tc_common.cuh"
 
 namespace usip {
 
-constexpr int TC_THREADS = 256;
-constexpr int TC_STAGES = 3;              // the stage-reuse argument above needs at least three
+constexpr int TC_CONSUMERS = 256;                    // two consumer warpgroups
+// + a producer warpgroup: with 384 threads a thread starts with 168 registers; the producer gives most of its share to the
+// consumers (40 + 2 x 232 per 128 threads), whose accumulators and two 3xTF32 A-fragment buffers need about 170
+constexpr int TC_THREADS = TC_CONSUMERS + 128;
+constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
 
 // ------------------------------------------------------------------------------------------------
 // weight pre-pack: W[Cout,Cin] (row stride ldw) -> per (n_tile, k_chunk) one contiguous, pre-swizzled block
-// [w_hi | w_lo] (TF32, BN x 128 B each, SWIZZLE_128B), so a stage's B operand is a single bulk copy.
+// [w_hi | w_lo] (TF32, BN x 128 B each, SWIZZLE_128B), K permuted as in the header, so a stage's B operand is a single
+// bulk copy.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tc_pack_one(const float* __restrict__ W, int ldw, int transposed, int Cout, int Cin, int BN,
                                             uint32_t* __restrict__ out, int t) {
   const int KC = Cin / TC_BK;
-  const int total = Cout * (Cin / 4);                 // one thread per 4 consecutive k
+  const int total = Cout * (Cin / 4);                 // one thread per 16-byte chunk of the packed row
   if (t >= total) return;
   const int n = t / (Cin / 4), k4 = t - n * (Cin / 4);
   const int kc = k4 / 8, c = k4 & 7;                  // 16-byte chunk c of K chunk kc
@@ -43,7 +55,8 @@ __device__ __forceinline__ void tc_pack_one(const float* __restrict__ W, int ldw
   uint32_t hi[4], lo[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    w[j] = transposed ? W[(size_t)(k4 * 4 + j) * ldw + n] : W[(size_t)n * ldw + k4 * 4 + j];
+    const int k = kc * TC_BK + 8 * j + c;             // logical column 4c + j <- physical column 8j + c
+    w[j] = transposed ? W[(size_t)k * ldw + n] : W[(size_t)n * ldw + k];
     split_tf32(w[j], hi[j], lo[j]);
   }
   const size_t blk = ((size_t)nt * KC + kc) * 2 * (size_t)BN * TC_BK;     // in 32-bit words
@@ -78,105 +91,132 @@ __global__ void tc_pack_many_kernel(const __grid_constant__ TcPackMany pm) {
 // ------------------------------------------------------------------------------------------------
 template <int BN>
 struct TcSmem {
-  static constexpr int A_STAGE = 2 * TC_BM * 128;                 // hi + lo
-  static constexpr int B_STAGE = 2 * BN * 128;
-  static constexpr int STAGE = A_STAGE + B_STAGE;
-  static constexpr int TILE = TC_BM * BN * 4;                    // epilogue staging tile, aliases the stages
-  static constexpr int COMB = 4 * 4 * BN * 4;                    // max, min, argmax, argmin per row quarter (group > 32 only)
-  static_assert(TILE + COMB <= TC_STAGES * STAGE, "epilogue tiles must fit in the stage memory");
-  static constexpr int BARS = 64;
-  static constexpr int BYTES = TC_STAGES * STAGE + BARS + 1024;  // +1024 alignment slack
+  static constexpr int STAGES = BN == 128 ? 4 : 8;               // weight ring: 128 KB of stages
+  static constexpr int B_STAGE = 2 * BN * 128;                   // [w_hi | w_lo] of one K chunk
+  static constexpr int TILE = TC_WG_ROWS * BN * 4;               // epilogue staging tile of one warpgroup
+  static constexpr int COMB = 4 * 4 * BN * 4;                    // max, min, argmax, argmin per 32-row quarter (group > 32)
+  static constexpr int BARS = 16 * STAGES;                       // full + empty barrier per stage
+  static constexpr int BYTES = STAGES * B_STAGE + 2 * TILE + 2 * COMB + BARS + 1024;   // +1024 alignment slack
 };
 
 // SINGLE: plain TF32, hi x hi only (the backward-precision option, usip_layer_desc.debug_flags & 8)
+// COMBINE: group-128 max/min; both warpgroups work on the halves of one 128-row tile and combine through shared memory
 template <int BN, bool COMBINE, bool SINGLE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 layer_fwd_tc_kernel(const usip_layer_desc d, const uint32_t* __restrict__ wpack) {
   using SM = TcSmem<BN>;
-  constexpr int S = TC_STAGES;
+  constexpr int S = SM::STAGES;
   constexpr int BK = TC_BK;                          // 32 floats per K chunk
-  constexpr int CPR = BK / 4;                        // 16-byte chunks per fp32 operand row
-  constexpr int RSTEP = TC_THREADS / CPR;            // rows covered by one pass of the CTA
-  constexpr int NJ = TC_BM / RSTEP;                  // float4 of X per thread and chunk
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-B alignment
   uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-  float* tile_s = reinterpret_cast<float*>(smem);
-  float* comb = reinterpret_cast<float*>(smem + SM::TILE);
-  const uint32_t bar_base = smem_base + S * SM::STAGE;
+  const uint32_t bar_base = smem_base + S * SM::B_STAGE + 2 * SM::TILE + 2 * SM::COMB;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto stage = [&](uint32_t it) { return smem_base + (it % S) * SM::STAGE; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int P = d.P, Cin = d.Cin, Cout = d.Cout;
-  const int KC = Cin / BK;
-  const int m_tiles = cdiv(P, TC_BM), n_tiles = Cout / BN;
-  const int num_tiles = m_tiles * n_tiles;
+  // warp index via a shuffle: the compiler then knows the role branches are warp-uniform (a branch it cannot prove uniform
+  // makes it serialise the wgmma)
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+  const int P = d.P, Cout = d.Cout;
+  const int KC = d.Cin / BK;
+  const bool ring = KC > S;                          // else the K panel is loaded once and stays resident
+  const int n_tiles = Cout / BN;
+  const int base = blockIdx.x / n_tiles, stride = gridDim.x / n_tiles;     // the grid is a multiple of n_tiles
+  const int nt = blockIdx.x - base * n_tiles, n0 = nt * BN;
+  // row tiles of this CTA: base, base + stride, ... (128-row tiles with COMBINE, else 64-row tiles)
+  const int cta_tiles = cdiv(cdiv(P, COMBINE ? TC_BM : TC_WG_ROWS) - base, stride);
 
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) mbar_init(full_bar(s), 1);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 2);                    // one arrival per warpgroup
+    }
     fence_barrier_init();
   }
   __syncthreads();
 
-  // ---- A producer: thread -> 16-byte chunk c of rows r0 + RSTEP*j
-  const int c = tid % CPR, r0 = tid / CPR;
+  // ================= producer warpgroup: one lane streams the column tile's K chunks through the ring, round after round
+  // (a round = one tile of each warpgroup; both read the same chunks).  In a round that only warpgroup 0 has a tile for,
+  // the producer arrives in warpgroup 1's place, after the stage's previous phase completed.
+  if (warp >= TC_CONSUMERS / 32) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (warp == TC_CONSUMERS / 32 && lane == 0) {
+      const int rounds = COMBINE ? cta_tiles : (cta_tiles + 1) / 2;
+      const int both = COMBINE ? cta_tiles : cta_tiles / 2;
+      const uint32_t* src = wpack + (size_t)nt * KC * 2 * BN * BK;
+      const int chunks = ring ? rounds * KC : KC;
+      for (int it = 0; it < chunks; ++it) {
+        const int s = it % S, kc = it % KC;
+        if (it >= S) mbar_wait_sleep(empty_bar(s), ((it / S) & 1) ^ 1);
+        mbar_arrive_expect_tx(full_bar(s), SM::B_STAGE);
+        bulk_g2s(smem_base + s * SM::B_STAGE, src + (size_t)kc * 2 * BN * BK, SM::B_STAGE, full_bar(s));
+        if (ring && it / KC >= both) mbar_arrive(empty_bar(s));
+      }
+    }
+    return;
+  }
+
+  // ================= consumer warpgroup wg
+  setmaxnreg_inc<TC_CONSUMER_REGS>();
+  const int wg = warp >> 2, wwarp = warp & 3, wtid = tid & 127;
+  const int my_tiles = COMBINE ? cta_tiles : (cta_tiles + 1 - wg) / 2;
+  auto tile_row0 = [&](int jt) {
+    return COMBINE ? (base + jt * stride) * TC_BM + TC_WG_ROWS * wg : (base + (2 * jt + wg) * stride) * TC_WG_ROWS;
+  };
+
+  // ---- A fragment: rows ra and ra + 8 of the tile, physical columns kq..kq+7 of each K chunk
+  const int ra = 16 * wwarp + (lane >> 2), kq = 8 * (lane & 3);
   const bool has_aff = d.in_scale != nullptr;
   const float relu_floor = d.in_relu ? 0.f : -INFINITY;
-  float4 xr[NJ], sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 xr[4];                                      // raw X of the next chunk: row ra (xr[0..1]), row ra + 8 (xr[2..3])
+  float4 sc[2] = {make_float4(1.f, 1.f, 1.f, 1.f), make_float4(1.f, 1.f, 1.f, 1.f)};
+  float4 sh[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
   auto fetch = [&](int row0, int kc) {
-    const int k = kc * BK + c * 4;
+    const int k = kc * BK + kq;
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int row = row0 + r0 + RSTEP * j;         // rows past P: zeros in, accumulator rows the epilogue never reads
-      xr[j] = row < P ? __ldg(reinterpret_cast<const float4*>(d.X + (size_t)row * d.ldx + k)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + ra + 8 * h;             // rows past P: zeros in, accumulator rows the epilogue never reads
+      if (row < P) {
+        const float4* p = reinterpret_cast<const float4*>(d.X + (size_t)row * d.ldx + k);
+        xr[2 * h] = __ldg(p); xr[2 * h + 1] = __ldg(p + 1);
+      } else {
+        xr[2 * h] = xr[2 * h + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
     }
-    if (has_aff) {                                   // the folded BN affine of these 4 input channels travels with the chunk
-      sc = __ldg(reinterpret_cast<const float4*>(d.in_scale + k));
-      sh = __ldg(reinterpret_cast<const float4*>(d.in_shift + k));
+    if (has_aff) {                                   // the folded BN affine of these 8 input channels travels with the chunk
+      sc[0] = __ldg(reinterpret_cast<const float4*>(d.in_scale + k)); sc[1] = __ldg(reinterpret_cast<const float4*>(d.in_scale + k + 4));
+      sh[0] = __ldg(reinterpret_cast<const float4*>(d.in_shift + k)); sh[1] = __ldg(reinterpret_cast<const float4*>(d.in_shift + k + 4));
     }
   };
   // hi = rna_tf32(v), lo = rna_tf32(v - hi): (bits + 0x1000) & ~0x1fff IS cvt.rna.tf32.f32 for finite inputs (round to
   // nearest, ties away, on the magnitude), without the inf/nan guard nvcc wraps around the cvt; activations here are finite.
-  auto split4 = [&](float v, uint32_t& hi, uint32_t& lo) {
-    hi = (__float_as_uint(v) + 0x1000u) & 0xffffe000u;
-    lo = (__float_as_uint(v - __uint_as_float(hi)) + 0x1000u) & 0xffffe000u;
-  };
-  auto store_a = [&](uint32_t a_hi) {
-    const uint32_t a_lo = a_hi + TC_BM * 128;
+  auto make_frag = [&](uint32_t (&hi)[16], uint32_t (&lo)[16]) {
+    const float s8[8] = {sc[0].x, sc[0].y, sc[0].z, sc[0].w, sc[1].x, sc[1].y, sc[1].z, sc[1].w};
+    const float h8[8] = {sh[0].x, sh[0].y, sh[0].z, sh[0].w, sh[1].x, sh[1].y, sh[1].z, sh[1].w};
+    const float x16[16] = {xr[0].x, xr[0].y, xr[0].z, xr[0].w, xr[1].x, xr[1].y, xr[1].z, xr[1].w,
+                           xr[2].x, xr[2].y, xr[2].z, xr[2].w, xr[3].x, xr[3].y, xr[3].z, xr[3].w};
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int r = r0 + RSTEP * j;
-      float v[4] = {xr[j].x, xr[j].y, xr[j].z, xr[j].w};
-      v[0] = fmaxf(fmaf(v[0], sc.x, sh.x), relu_floor); v[1] = fmaxf(fmaf(v[1], sc.y, sh.y), relu_floor);
-      v[2] = fmaxf(fmaf(v[2], sc.z, sh.z), relu_floor); v[3] = fmaxf(fmaf(v[3], sc.w, sh.w), relu_floor);
-      uint32_t hi[4], lo[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) split4(v[q], hi[q], lo[q]);
-      const uint32_t off = (uint32_t)r * 128u + (uint32_t)((c ^ (r & 7)) << 4);
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_hi + off), "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]) : "memory");
-      if (!SINGLE)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_lo + off), "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]) : "memory");
+    for (int i = 0; i < 16; ++i) {
+      // physical column 2s + b of row half h is k-step s, register 2b + h
+      const int h = i >> 3, s = (i & 7) >> 1, b = i & 1;
+      const float v = fmaxf(fmaf(x16[i], s8[i & 7], h8[i & 7]), relu_floor);
+      const uint32_t vh = (__float_as_uint(v) + 0x1000u) & 0xffffe000u;
+      hi[4 * s + 2 * b + h] = vh;
+      lo[4 * s + 2 * b + h] = (__float_as_uint(v - __uint_as_float(vh)) + 0x1000u) & 0xffffe000u;
     }
   };
-  // ---- B operand: one bulk copy of the packed [w_hi | w_lo] tile, completion counted on the stage's barrier (thread 0)
-  auto issue_b = [&](uint32_t it, int nt, int kc) {
-    const uint32_t s = it % S;
-    mbar_arrive_expect_tx(full_bar(s), SM::B_STAGE);
-    bulk_g2s(stage(it) + SM::A_STAGE, wpack + ((size_t)nt * KC + kc) * 2 * (size_t)BN * BK, SM::B_STAGE, full_bar(s));
-  };
 
-  // ---- epilogue role: warp -> 32-row quarter q of the tile (rows 32q..32q+31), chunks with (ch & 1) == half
-  const int q = warp & 3, half = warp >> 2;
+  // ---- epilogue role: warp -> 32-row quarter q of the warpgroup tile, column chunks with (ch & 1) == half
+  const int q = wwarp & 1, half = wwarp >> 1;
   const int g = d.group;
   const bool want_stats = d.stat_partial != nullptr;
   const bool want_grp = (d.gmax != nullptr) || (d.gmin != nullptr);
-  // BN statistics: ONE partial row per (CTA, row quarter), accumulated over the CTA's tiles.  The grid is a multiple of
-  // n_tiles, so a CTA always works on the same column tile and column (slot, c) belongs to exactly one lane of one warp
-  // for the whole kernel: a plain read-modify-write of an L2-resident float, first tile stores.
-  float* stat_row = want_stats ? d.stat_partial + ((size_t)(blockIdx.x / n_tiles) * 4 + q) * 2 * Cout : nullptr;
-  int tcount = 0;
-  auto stat_accumulate = [&](int col, float s, float ss) {
+  float* tile_s = reinterpret_cast<float*>(smem + S * SM::B_STAGE + wg * SM::TILE);
+  // BN statistics: ONE partial row per (CTA, warpgroup, row quarter), accumulated over the warpgroup's tiles.  A CTA keeps
+  // its column tile, so column (slot, c) belongs to exactly one lane of one warp for the whole kernel: a plain
+  // read-modify-write of an L2-resident float, first tile stores.
+  float* stat_row = want_stats ? d.stat_partial + ((size_t)base * 4 + 2 * wg + q) * 2 * Cout : nullptr;
+  auto stat_accumulate = [&](int tcount, int col, float s, float ss) {
     float* ps = stat_row + col;
     float* pq = stat_row + Cout + col;
     if (tcount != 0) { s += *ps; ss += *pq; }
@@ -184,41 +224,33 @@ layer_fwd_tc_kernel(const usip_layer_desc d, const uint32_t* __restrict__ wpack)
   };
 
   float acc[BN / 2];
-  uint32_t it = 0;                                   // chunks issued by this CTA: stage it % S, barrier parity (it / S) & 1
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tcount) {
-    const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-    const int row0 = mt * TC_BM, n0 = nt * BN;
-    // ================= main loop (all stages are idle here: the previous tile ended with a CTA barrier)
-    if (tid == 0) {
-      fence_proxy_async_smem();                      // the epilogue's generic-proxy use of this memory precedes the TMA writes
-      issue_b(it, nt, 0);
-      if (KC > 1) issue_b(it + 1, nt, 1);
-    }
-    fetch(row0, 0);
-    store_a(stage(it));
-    if (KC > 1) fetch(row0, 1);
-    fence_proxy_async_smem();                        // generic-proxy writes -> visible to wgmma (async proxy)
-    __syncthreads();
-    for (int kc = 0; kc < KC; ++kc, ++it) {
+  uint32_t fh0[16], fl0[16], fh1[16], fl1[16];       // A fragments of even / odd chunks
+  if (my_tiles > 0) fetch(tile_row0(0), 0);
+  for (int jt = 0; jt < my_tiles; ++jt) {
+    const int row0 = tile_row0(jt);
+    // ================= main loop over the tile's K chunks
+    auto step = [&](uint32_t (&fh)[16], uint32_t (&fl)[16], int kc) {
+      make_frag(fh, fl);                             // the last reader of fh / fl, chunk kc - 2, retired
+      if (kc + 1 < KC) fetch(row0, kc + 1);
+      else if (jt + 1 < my_tiles) fetch(tile_row0(jt + 1), 0);
+      const int it = ring ? jt * KC + kc : kc;       // ring position: stage it % S, phase parity (it / S) & 1
       mbar_wait(full_bar(it % S), (it / S) & 1);
-      const uint32_t a_hi = stage(it) + (warp >> 2) * 64 * 128, b_hi = stage(it) + SM::A_STAGE;
-      wgmma_chunk<BN, SINGLE>(acc, a_hi, a_hi + TC_BM * 128, b_hi, b_hi + BN * 128, kc == 0);
-      wgmma_wait<1>();                               // this warpgroup's chunk it-1 retired
-      if (kc + 1 < KC) {
-        store_a(stage(it + 1));                      // stage of chunk it-2: retired in both warpgroups
-        if (kc + 2 < KC) fetch(row0, kc + 2);
-        fence_proxy_async_smem();
-      }
-      __syncthreads();
-      if (tid == 0 && kc + 2 < KC) issue_b(it + 2, nt, kc + 2);   // stage of chunk it-1: retired in both warpgroups
+      wgmma_chunk_rs<BN, SINGLE>(acc, fh, fl, smem_base + (it % S) * SM::B_STAGE, kc == 0);
+      wgmma_wait<1>();                               // chunk kc - 1 retired
+      if (ring && kc > 0 && wtid == 0) mbar_arrive(empty_bar((it - 1) % S));
+    };
+#pragma unroll 1
+    for (int kc = 0; kc < KC; kc += 2) {
+      step(fh0, fl0, kc);
+      if (kc + 1 < KC) step(fh1, fl1, kc + 1);
     }
     wgmma_wait<0>();
     wgmma_fence_acc(acc);
-    __syncthreads();                                 // no wgmma reads the stages any more: they become the staging tile
+    if (ring && wtid == 0) mbar_arrive(empty_bar((jt * KC + KC - 1) % S));
 
     // ================= accumulators (+addend, +bias) -> staging tile, element (r, c) at r*BN + (((c>>2) ^ (r&7))<<2) + (c&3)
+    named_bar_sync(1 + wg, 128);                     // this warpgroup finished reading its previous tile's staging
     {
-      const int ra = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = ra + 8 * h, row = row0 + r;
@@ -238,9 +270,13 @@ layer_fwd_tc_kernel(const usip_layer_desc d, const uint32_t* __restrict__ wpack)
         }
       }
     }
-    __syncthreads();
+    named_bar_sync(1 + wg, 128);
 
-    // ================= epilogue: warp (q, half) on the 32 x 32 chunks of rows 32q..32q+31
+    // ================= epilogue: warp (q, half) on the 32 x 32 chunks of rows 32q..32q+31 of the warpgroup tile
+    // group > 32: per-quarter results go to comb[kind][quarter of the 128-row tile][column]; with COMBINE the buffer
+    // alternates with the tile so that one warpgroup's next tile cannot overwrite what the other still reads
+    float* comb = reinterpret_cast<float*>(smem + S * SM::B_STAGE + 2 * SM::TILE + (COMBINE ? (jt & 1) : 0) * SM::COMB);
+    const int cq = 2 * wg + q;                       // quarter slot in comb
     const int wrow0 = row0 + q * 32;                 // first row of this warp
     const int nvalid = min(32, max(0, P - wrow0));   // valid rows of this warp
 #pragma unroll 1
@@ -274,7 +310,7 @@ layer_fwd_tc_kernel(const usip_layer_desc d, const uint32_t* __restrict__ wpack)
         } else {
           for (int r = 0; r < nvalid; ++r) { const float x0 = tw[r * BN + ((cchunk ^ (r & 7)) << 2) + csub]; s0 += x0; q0 = fmaf(x0, x0, q0); }
         }
-        stat_accumulate(cb + lane, s0 + s1, q0 + q1);
+        stat_accumulate(jt, cb + lane, s0 + s1, q0 + q1);
       } else if (want_grp) {
         float s = 0.f, ss = 0.f;
         float mx0 = -INFINITY, mn0 = INFINITY, mx1 = -INFINITY, mn1 = INFINITY;
@@ -308,7 +344,7 @@ layer_fwd_tc_kernel(const usip_layer_desc d, const uint32_t* __restrict__ wpack)
             }
           }
         }
-        if (want_stats) stat_accumulate(cb + lane, s, ss);
+        if (want_stats) stat_accumulate(jt, cb + lane, s, ss);
         if (g == 16) {
           const int grow = wrow0 / 16;
           if (nvalid > 0) {
@@ -331,35 +367,37 @@ layer_fwd_tc_kernel(const usip_layer_desc d, const uint32_t* __restrict__ wpack)
             if (d.garg_max) d.garg_max[(size_t)grow * Cout + cb + lane] = ax0;
             if (d.garg_min) d.garg_min[(size_t)grow * Cout + cb + lane] = an0;
           }
-        } else if (COMBINE) {                       // 64 / 128: combine the row quarters below
-          comb[(0 * 4 + q) * BN + cl] = mx0; comb[(1 * 4 + q) * BN + cl] = mn0;
-          reinterpret_cast<int*>(comb)[(2 * 4 + q) * BN + cl] = q * 32 + ax0;
-          reinterpret_cast<int*>(comb)[(3 * 4 + q) * BN + cl] = q * 32 + an0;
+        } else {                                     // 64 / 128: combine the row quarters below
+          const int qoff = (COMBINE ? cq : q) * 32;  // first row of this quarter inside the group
+          comb[(0 * 4 + cq) * BN + cl] = mx0; comb[(1 * 4 + cq) * BN + cl] = mn0;
+          reinterpret_cast<int*>(comb)[(2 * 4 + cq) * BN + cl] = qoff + ax0;
+          reinterpret_cast<int*>(comb)[(3 * 4 + cq) * BN + cl] = qoff + an0;
         }
       }
     }
-    if (COMBINE && want_grp && g > 32) {
-      __syncthreads();
-      const int wpg = g / 32;                        // row quarters per group: 2 or 4
-      for (int cl = tid; cl < BN; cl += TC_THREADS) {
-        for (int gi = 0; gi < 4 / wpg; ++gi) {
-          const int grow = row0 / g + gi;
-          if ((size_t)grow * g >= (size_t)P) break;
-          float mx = -INFINITY, mn = INFINITY; int ax = 0, an = 0;
-          for (int w = gi * wpg; w < (gi + 1) * wpg; ++w) {
-            const float a = comb[(0 * 4 + w) * BN + cl], b = comb[(1 * 4 + w) * BN + cl];
-            if (a > mx) { mx = a; ax = reinterpret_cast<int*>(comb)[(2 * 4 + w) * BN + cl]; }
-            if (b < mn) { mn = b; an = reinterpret_cast<int*>(comb)[(3 * 4 + w) * BN + cl]; }
-          }
-          if (d.gmax) d.gmax[(size_t)grow * Cout + n0 + cl] = mx;
-          if (d.gmin) d.gmin[(size_t)grow * Cout + n0 + cl] = mn;
-          if (d.garg_max) d.garg_max[(size_t)grow * Cout + n0 + cl] = ax - gi * g;
-          if (d.garg_min) d.garg_min[(size_t)grow * Cout + n0 + cl] = an - gi * g;
+    if (want_grp && g > 32) {
+      // group 64 is this warpgroup's tile (quarters 2wg, 2wg + 1); group 128 (COMBINE) is both warpgroups' tiles
+      if (COMBINE) named_bar_sync(3, TC_CONSUMERS);
+      else named_bar_sync(1 + wg, 128);
+      const int q0 = COMBINE ? 0 : 2 * wg, nq = COMBINE ? 4 : 2;
+      const int grow = row0 / g;
+      for (int cl = COMBINE ? tid : wtid; cl < BN; cl += COMBINE ? TC_CONSUMERS : 128) {
+        float mx = -INFINITY, mn = INFINITY; int ax = 0, an = 0;
+        for (int w = q0; w < q0 + nq; ++w) {
+          const float a = comb[(0 * 4 + w) * BN + cl], b = comb[(1 * 4 + w) * BN + cl];
+          if (a > mx) { mx = a; ax = reinterpret_cast<int*>(comb)[(2 * 4 + w) * BN + cl]; }
+          if (b < mn) { mn = b; an = reinterpret_cast<int*>(comb)[(3 * 4 + w) * BN + cl]; }
         }
+        if (d.gmax) d.gmax[(size_t)grow * Cout + n0 + cl] = mx;
+        if (d.gmin) d.gmin[(size_t)grow * Cout + n0 + cl] = mn;
+        if (d.garg_max) d.garg_max[(size_t)grow * Cout + n0 + cl] = ax;
+        if (d.garg_min) d.garg_min[(size_t)grow * Cout + n0 + cl] = an;
       }
     }
-    __syncthreads();                                 // the next tile's A / B writes reuse the staging memory
   }
+  // a warpgroup without a tile (a CTA with a single 64-row tile) still owns its statistic slots: they sum to zero
+  if (want_stats && my_tiles == 0)
+    for (int ch = half; ch < BN / 32; ch += 2) stat_accumulate(0, n0 + ch * 32 + lane, 0.f, 0.f);
 }
 
 // persistent grid: one CTA per SM, rounded down to a multiple of the column-tile count so that a CTA keeps its column
@@ -393,7 +431,9 @@ static int tc_pick_bn(const usip_layer_desc& d) {
   return 64;
 }
 
-// number of [2, Cout] BN-statistic partial rows usip_layer_fwd writes for this descriptor (tensor-core precisions)
+// number of [2, Cout] BN-statistic partial rows usip_layer_fwd writes for this descriptor (tensor-core precisions): one
+// per (CTA row base = blockIdx.x / n_tiles, warpgroup, 32-row quarter of the warpgroup tile), slot base*4 + 2*wg + q;
+// the n_tiles CTAs of one base fill disjoint column ranges of the same four slots
 int tc_stat_slots(const usip_layer_desc& d) {
   const int BN = tc_pick_bn(d);
   return tc_grid(d.P, d.Cout, BN, device_sm_count()) / (d.Cout / BN) * 4;
@@ -442,7 +482,7 @@ int layer_fwd_tc(const usip_layer_desc& d, cudaStream_t st) {
     int e = check_launch("tc_pack_weights_kernel");
     if (e) return e;
   }
-  const bool combine = (d.gmax || d.gmin) && d.group > 32;
+  const bool combine = (d.gmax || d.gmin) && d.group == 128;      // groups of 16..64 rows lie inside a warpgroup tile
   if (d.debug_flags & 8) {
     if (combine) return BN == 128 ? launch_tc<128, true, true>(d, wpack, st) : launch_tc<64, true, true>(d, wpack, st);
     return BN == 128 ? launch_tc<128, false, true>(d, wpack, st) : launch_tc<64, false, true>(d, wpack, st);

@@ -5,6 +5,7 @@
 namespace usip {
 
 constexpr int TC_BM = 128;                 // rows per CTA tile: two warpgroups, one m64 wgmma row block each
+constexpr int TC_WG_ROWS = 64;             // rows per warpgroup tile of the layer kernel (one m64 wgmma row block)
 constexpr int TC_BK = 32;                  // floats per K chunk (= one 128-byte swizzle row)
 
 // ------------------------------------------------------------------------------------------------ PTX
@@ -46,6 +47,14 @@ __device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity) {
       : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// per-thread register budget of the executing warpgroup (all its warps execute it): hands registers from a producer
+// warpgroup to the consumers
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+// barrier `id` (1..15; 0 is __syncthreads) over `threads` threads, a multiple of 32: couples only the warps that use it
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
@@ -159,6 +168,79 @@ __device__ __forceinline__ void wgmma_chunk(float (&d)[BN / 2], uint32_t a_hi, u
       wgmma_tf32<BN>(d, make_kmajor_sw128_desc(a_lo + ks * 32), dbh, acc);
       wgmma_tf32<BN>(d, dah, make_kmajor_sw128_desc(b_lo + ks * 32), 1u);
       wgmma_tf32<BN>(d, dah, dbh, 1u);
+    }
+  }
+  wgmma_commit();
+  wgmma_fence_acc(d);
+}
+
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T with A in registers (B as above).  A fragment of lane l of warp w of the warpgroup:
+// a[0] = (row 16w + l/4, k l%4), a[1] = (row 16w + l/4 + 8, k l%4), a[2] = (row 16w + l/4, k l%4 + 4),
+// a[3] = (row 16w + l/4 + 8, k l%4 + 4).  The registers must not change until the wgmma group that reads them retired.
+__device__ __forceinline__ void wgmma_tf32_rs_n64(float (&d)[32], const uint32_t* a, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accum)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_rs_n128(float (&d)[64], const uint32_t* a, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %69, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accum)
+      : "memory");
+}
+
+// wgmma_chunk with the warpgroup's A fragments in registers: a_*[4ks .. 4ks+3] is the fragment of k-step ks.  b_hi points
+// at the stage's [b_hi | b_lo] tile.  With SINGLE, a_lo is not read.
+template <int BN, bool SINGLE>
+__device__ __forceinline__ void wgmma_chunk_rs(float (&d)[BN / 2], const uint32_t (&a_hi)[16], const uint32_t (&a_lo)[16],
+                                               uint32_t b_hi, bool first) {
+  static_assert(BN == 64 || BN == 128, "wgmma tile width");
+  const uint32_t b_lo = b_hi + BN * 128;
+  wgmma_fence_acc(d);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < TC_BK / 8; ++ks) {
+    const uint64_t dbh = make_kmajor_sw128_desc(b_hi + ks * 32);
+    const uint32_t acc = (first && ks == 0) ? 0u : 1u;
+    auto mma = [&](const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
+      if constexpr (BN == 64) wgmma_tf32_rs_n64(d, a, bdesc, scale_d);
+      else wgmma_tf32_rs_n128(d, a, bdesc, scale_d);
+    };
+    if constexpr (SINGLE) {
+      mma(a_hi + 4 * ks, dbh, acc);
+    } else {
+      mma(a_lo + 4 * ks, dbh, acc);
+      mma(a_hi + 4 * ks, make_kmajor_sw128_desc(b_lo + ks * 32), 1u);
+      mma(a_hi + 4 * ks, dbh, 1u);
     }
   }
   wgmma_commit();
