@@ -20,7 +20,6 @@
 // more than 64 hits, K > 64 and non-finite radii take the reference's own in-order scan (bit-identical by construction).
 #include "tc_common.cuh"
 #include <cstdlib>
-#include <cuda.h>           // CUtensorMap types only; the encoder is resolved at run time
 
 namespace usip {
 
@@ -334,28 +333,13 @@ bx_query_kernel(const __grid_constant__ CUtensorMap tmap, const float* __restric
 float radius_to_tmax_host(float radius);          // ballquery.cu
 
 // Tensor map of the bucket planes: 3-D tensor [B clouds][BX_ROWS rows][BX_PITCH cells x 64 floats], box = 3 cells x 3 rows.
-// cuTensorMapEncodeTiled is resolved through the runtime (cudaGetDriverEntryPoint): the library keeps no link-time
-// dependency on libcuda, so it still loads (and exports its symbols) on a machine without a driver.
 static int bx_tensor_map(CUtensorMap* tm, float4* buckets, int B) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
-    if (e != cudaSuccess || !fn) { set_last_error("ball_group: cuTensorMapEncodeTiled not available"); return e != cudaSuccess ? (int)e : -1; }
-    encode = (EncodeFn)fn;
-  }
   const cuuint64_t dims[3] = {(cuuint64_t)BX_PITCH * BX_CAP * 8, (cuuint64_t)BX_ROWS, (cuuint64_t)B};
   const cuuint64_t strides[2] = {(cuuint64_t)BX_PITCH * BX_CAP * 32, (cuuint64_t)BX_MAX_CELLS * BX_CAP * 32};   // bytes, dims 1..2
   const cuuint32_t box[3] = {3 * BX_CAP * 8, 3, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, buckets, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error("ball_group: cuTensorMapEncodeTiled failed"); return (int)r; }
-  return 0;
+  return encode_tensor_map_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, buckets, dims, strides, box, estr,
+                                 CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, "ball_group: bucket tensor map");
 }
 
 }  // namespace usip

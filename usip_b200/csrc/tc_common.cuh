@@ -1,6 +1,8 @@
-// tc_common.cuh -- PTX wrappers shared by the Hopper tensor-core kernels (mbarrier, TMA bulk copy, wgmma descriptors).
+// tc_common.cuh -- PTX wrappers shared by the Hopper tensor-core kernels (mbarrier, TMA bulk copy, wgmma descriptors) and
+// the host-side tensor-map encoder.
 #pragma once
 #include "common.cuh"
+#include <cuda.h>           // CUtensorMap types only; the encoder is resolved at run time
 
 namespace usip {
 
@@ -61,6 +63,40 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
+}
+// box {c0.., c1..} of a 2-D tensor map (a __grid_constant__ parameter) -> shared memory.  Elements past the tensor's
+// bounds arrive as zeros, and the barrier's transaction still counts the whole box.
+__device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+               ::"r"(dst_smem), "l"(map), "r"(c0), "r"(c1), "r"(bar)
+               : "memory");
+}
+__device__ __forceinline__ void prefetch_tensor_map(const CUtensorMap* map) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+
+// cuTensorMapEncodeTiled (no interleave, out-of-bounds elements read as zeros), resolved once through the runtime
+// (cudaGetDriverEntryPoint): the library keeps no link-time dependency on libcuda, so it still loads (and exports its
+// symbols) on a machine without a driver.  Returns 0, or an error code with the last error set to `what`.
+inline int encode_tensor_map_tiled(CUtensorMap* tm, CUtensorMapDataType dtype, cuuint32_t rank, void* gaddr,
+                                   const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box,
+                                   const cuuint32_t* estr, CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2,
+                                   const char* what) {
+  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static EncodeFn encode = nullptr;
+  if (!encode) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
+    if (e != cudaSuccess || !fn) { set_last_error(what); return e != cudaSuccess ? (int)e : -1; }
+    encode = (EncodeFn)fn;
+  }
+  CUresult r = encode(tm, dtype, rank, gaddr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_last_error(what); return (int)r; }
+  return 0;
 }
 
 __device__ __forceinline__ uint32_t to_tf32(float x) {
