@@ -75,7 +75,50 @@ int usip_knn_group_f32(const float* xyz, const float* feat, const float* centers
 int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float* out_nodes, int B, int Ns, int k,
                  void* stream);
 
-/* Radius non-maximum suppression of the detected keypoints     evaluation/save_keypoints.py:180-216 (nms)
+/* Detector training pairs on the device (csrc/pairgen.cu)  data/kitti_detector_loader.py:101-259 (KittiLoader.__getitem__)
+ * Input: a ragged batch of raw scans, scans [T, C] f32 (x, y, z, then C-3 feature columns) with row offsets (n_scans+1)
+ * i64; scan_of_pair (n_pairs) i32 names the scan of every pair.  Clouds are numbered c = 2*pair + side (0 = src, 1 = dst),
+ * both sides subsample the same scan independently.  Every per-point random number is Philox4x32-10 keyed by
+ * (seed, step, cloud, point, purpose), so a batch is a pure function of (seed, step).
+ *
+ * usip_pair_subsample (get_instance_unaugmented_np, :118-145):
+ *   out_rows (2*n_pairs, N) i32: row indices into each cloud's scan.  Optional radius mask (use_radius): fp32
+ *     sqrt(x*x + z*z) compared in double against `radius`.  >= N points inside: a uniform subset of N without
+ *     replacement, ascending row index.  Ns < N inside: every inside row t times (t the smallest >= 1 with Ns + t*Ns >= N),
+ *     ascending, then a uniform subset of the N - t*Ns remainder, ascending.  A scan with no point inside gets rows 0.
+ *   out_cand (2*n_pairs, n_cand) i32: a uniform subset of n_cand of the N positions, ascending (the FPS candidates).
+ *   out_start (2*n_pairs) i32: the FPS start index in [0, n_cand).  out_valid (2*n_pairs) i32: points inside (or NULL).
+ *   max_rows >= the longest scan; max(max_rows, N) <= usip_pair_max_scan_rows().
+ * usip_pair_gather_candidates: out_pts (2*n_pairs, n_cand, 3) f32 = xyz of rows[c, cand[c, j]] -- usip_fps_f32's input.
+ * usip_pair_augment (augment(), :149-216, train mode only, then transform_pc_pytorch for dst, augmentation.py:199-248):
+ *   rows as above, nodes (2*n_pairs, 3, M) f32 = the FPS nodes (usip_fps_f32 out_nodes);
+ *   params (n_pairs, 48) f64 per pair: [0:9] horizontal, [9:18] 3-d and [18:27] perturbation rotation matrices (row
+ *     major, applied as data @ R in float64), [27] augmentation scale, [28:31] augmentation shift, [31:40] the transform's
+ *     R (fp32 values), [40:43] its shift, [43] its scale;
+ *   jit_pc (2*n_pairs, N, 3), jit_sn (2*n_pairs, N, S), jit_node (2*n_pairs, M, 3) f64 clipped jitter, each NULL to draw
+ *     it on the device (N(0, 0.04^2) clipped at 0.12 for pc / node, N(0, 0.01^2) clipped at 0.05 for sn);
+ *   flags: USIP_PAIR_* below.  sn = columns 3:3+S of the scan, or the last column when S == 1.
+ *   -> src/dst pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M), R (n_pairs, 3, 3), scale (n_pairs),
+ *      shift (n_pairs, 3, 1), all f32 -- the nine tensors of ModelDetector.set_input. */
+#define USIP_PAIR_TRAIN 1
+#define USIP_PAIR_ROT_HORIZONTAL 2
+#define USIP_PAIR_ROT_3D 4
+#define USIP_PAIR_ROT_PERTURBATION 8
+#define USIP_PAIR_TRANSLATION 16
+int usip_pair_max_scan_rows(void);
+int usip_pair_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair, int max_rows,
+                        int n_pairs, int N, int n_cand, int use_radius, double radius, uint64_t seed, uint64_t step,
+                        int32_t* out_rows, int32_t* out_cand, int32_t* out_start, int32_t* out_valid, void* stream);
+int usip_pair_gather_candidates(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,
+                                const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
+                                int n_cand, void* stream);
+int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,
+                      const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
+                      const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
+                      int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node, float* dst_pc,
+                      float* dst_sn, float* dst_node, float* R, float* scale, float* shift, void* stream);
+
+/* Radius non-maximum suppression of the detected keypoints    evaluation/save_keypoints.py:180-216 (nms)
  * keypoints (B,3,M) f32, sigmas (B,M) f32 -> out_idx (B,M) i32: original indices of the kept keypoints in the order the
  * reference emits them (ascending sigma, ties by index), padded with -1; out_count (B,) i32.  radius < 0.01: pass-through
  * (0..M-1, count M) like the reference. */

@@ -320,6 +320,46 @@ def golden_nms(ref):
     np.savez_compressed(os.path.join(OUT, "nms.npz"), **out)
 
 
+# data/kitti_detector_loader.py KittiLoader.__getitem__ on a synthetic KITTI tree (usip_b200.data.kitti_detector_loader.
+# write_synthetic_kitti): train sequences 0..8, test sequences 9..10, every scan (PAIRS_NS, 8) float32.
+PAIRS_COUNTS = [2, 1, 1, 1, 1, 1, 1, 1, 2, 1, 2]
+PAIRS_NS, PAIRS_TREE_SEED = 1300, 7100
+PAIRS_CASES = {     # name: (mode, index, np seed, S, rot_horizontal, rot_3d, rot_perturbation, translation, radius)
+    "kitti": ("train", 3, 11, 4, 1, 0, 0, 0, 100.0),
+    "s1": ("train", 0, 12, 1, 1, 0, 0, 0, 100.0),
+    "s5": ("train", 10, 13, 5, 1, 0, 0, 0, 100.0),
+    "rot3d": ("train", 5, 14, 3, 0, 1, 1, 1, 100.0),
+    "radius": ("train", 1, 15, 4, 1, 0, 0, 0, 20.0),
+    "test": ("test", 2, 16, 4, 1, 0, 0, 0, 100.0),
+}
+
+
+def golden_pairs(ref):
+    import importlib
+    import tempfile
+    from usip_b200.data.kitti_detector_loader import write_synthetic_kitti
+    kl = importlib.import_module("data.kitti_detector_loader")
+    out = {"tree/counts": np.array(PAIRS_COUNTS), "tree/Ns": np.int64(PAIRS_NS), "tree/seed": np.int64(PAIRS_TREE_SEED),
+           "N": np.int64(1024), "M": np.int64(64)}
+    keys = ("src_pc", "src_sn", "src_node", "dst_pc", "dst_sn", "dst_node", "R", "scale", "shift")
+    with tempfile.TemporaryDirectory() as root:
+        write_synthetic_kitti(root, PAIRS_COUNTS, PAIRS_NS, seed=PAIRS_TREE_SEED)
+        for name, (mode, index, seed, S, rh, r3, rp, tp, radius) in PAIRS_CASES.items():
+            opt = ref_shim.make_opt(input_pc_num=1024, node_num=64, surface_normal_len=S, rot_horizontal=bool(rh),
+                                    rot_3d=bool(r3), rot_perturbation=bool(rp), translation_perturbation=bool(tp),
+                                    radius_threshold=radius)
+            loader = kl.KittiLoader(root, mode, opt)
+            np.random.seed(seed)
+            res = loader[index]
+            out[name + "/case"] = np.array([index, seed, S, rh, r3, rp, tp], dtype=np.int64)
+            out[name + "/mode"] = np.array(mode)
+            out[name + "/radius"] = np.float64(radius)
+            for k, v in zip(keys, res):
+                out[name + "/" + k] = np.asarray(v.numpy() if torch.is_tensor(v) else v, dtype=np.float32)
+            print("pairs", name, {k: out[name + "/" + k].shape for k in keys})
+    np.savez_compressed(os.path.join(OUT, "detector_pairs.npz"), **out)
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)

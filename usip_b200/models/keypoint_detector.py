@@ -103,13 +103,16 @@ class ModelDetector():
             setattr(self, k, a.float().to(dev, non_blocking=True).detach())
         torch.cuda.synchronize()                                  # keypoint_detector.py:134
 
-    def prefetch_input(self, *args):
+    def prefetch_input(self, *args, after=None):
         """Not in the reference: stage the NEXT batch (same nine tensors as set_input, ideally pinned) with asynchronous
         host-to-device copies on a dedicated stream, so that the transfer overlaps the step that is running.  The
-        following set_input() with the same tensor objects adopts the staged copies."""
+        following set_input() with the same tensor objects adopts the staged copies.  `after`: a CUDA event the staging
+        waits for (device tensors produced on another stream, e.g. by DetectorPairBuilder)."""
         dev = self.opt.device
         if getattr(self, "_copy_stream", None) is None:
             self._copy_stream = torch.cuda.Stream(device=dev)
+        if after is not None:
+            self._copy_stream.wait_event(after)
         with torch.cuda.stream(self._copy_stream):
             staged = [a.float().to(dev, non_blocking=True).detach() for a in args]
             ev = torch.cuda.Event()

@@ -137,6 +137,71 @@ def fps(pts, start, k, want_nodes=True):
     return idx, nodes
 
 
+# --------------------------------------------------------------------------- detector training pairs (csrc/pairgen.cu)
+PAIR_TRAIN, PAIR_ROT_HORIZONTAL, PAIR_ROT_3D, PAIR_ROT_PERTURBATION, PAIR_TRANSLATION = 1, 2, 4, 8, 16
+PAIR_PARAM_STRIDE = 48
+
+
+def pair_max_scan_rows():
+    return _lib.load().usip_pair_max_scan_rows()
+
+
+def _req_scans(scans, offsets, scan_of_pair):
+    _req(scans, f32, "scans"); _req(offsets, torch.int64, "offsets"); _req(scan_of_pair, i32, "scan_of_pair")
+    if scans.dim() != 2 or scans.shape[1] < 3:
+        raise ValueError("scans must be [T, C] with C >= 3")
+
+
+def pair_subsample(scans, offsets, scan_of_pair, max_rows, N, n_cand, radius=None, seed=0, step=0):
+    """Device-mode subsets.  scans [T, C] f32, offsets (n_scans+1,) i64, scan_of_pair (B,) i32 ->
+    rows (2B, N) i32, cand (2B, n_cand) i32, start (2B,) i32, valid (2B,) i32 (points inside the radius)."""
+    _req_scans(scans, offsets, scan_of_pair)
+    B, dev = scan_of_pair.shape[0], scans.device
+    rows = torch.empty((2 * B, int(N)), dtype=i32, device=dev)
+    cand = torch.empty((2 * B, int(n_cand)), dtype=i32, device=dev)
+    start = torch.empty((2 * B,), dtype=i32, device=dev)
+    valid = torch.empty((2 * B,), dtype=i32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_pair_subsample(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_pair), int(max_rows), B, int(N), int(n_cand),
+            int(radius is not None), float(radius if radius is not None else 0.0), int(seed) & (2 ** 64 - 1),
+            int(step) & (2 ** 64 - 1), _p(rows), _p(cand), _p(start), _p(valid), _stream()), "usip_pair_subsample")
+    return rows, cand, start, valid
+
+
+def pair_gather_candidates(scans, offsets, scan_of_pair, rows, cand):
+    """FPS input: (2B, n_cand, 3) f32 xyz of rows[c, cand[c, j]]."""
+    _req_scans(scans, offsets, scan_of_pair); _req(rows, i32, "rows"); _req(cand, i32, "cand")
+    B, N, n_cand = scan_of_pair.shape[0], rows.shape[1], cand.shape[1]
+    pts = torch.empty((2 * B, n_cand, 3), dtype=f32, device=scans.device)
+    with torch.cuda.device(scans.device):
+        check(_lib.load().usip_pair_gather_candidates(_p(scans), scans.shape[1], _p(offsets), _p(scan_of_pair), _p(rows),
+                                                      _p(cand), _p(pts), B, N, n_cand, _stream()),
+              "usip_pair_gather_candidates")
+    return pts
+
+
+def pair_augment(scans, offsets, scan_of_pair, rows, nodes, params, S, flags, seed=0, step=0, jit_pc=None, jit_sn=None,
+                 jit_node=None):
+    """Augmentation + dst transform -> the nine ModelDetector.set_input tensors (src_pc, src_sn, src_node, dst_pc,
+    dst_sn, dst_node, R, scale, shift).  params (B, 48) f64 on the device (layout in include/usip_b200.h); jitter arrays
+    f64 or None (drawn on the device from (seed, step))."""
+    _req_scans(scans, offsets, scan_of_pair); _req(rows, i32, "rows"); _req(nodes, f32, "nodes")
+    _req(params, torch.float64, "params")
+    for name, j in (("jit_pc", jit_pc), ("jit_sn", jit_sn), ("jit_node", jit_node)):
+        if j is not None:
+            _req(j, torch.float64, name)
+    B, N, M, dev = scan_of_pair.shape[0], rows.shape[1], nodes.shape[2], scans.device
+    e = lambda *s: torch.empty(s, dtype=f32, device=dev)
+    out = (e(B, 3, N), e(B, S, N), e(B, 3, M), e(B, 3, N), e(B, S, N), e(B, 3, M), e(B, 3, 3), e(B), e(B, 3, 1))
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_pair_augment(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_pair), _p(rows), _p(nodes), _p(params), _p(jit_pc),
+            _p(jit_sn), _p(jit_node), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), int(flags), int(S), B, N, M,
+            *[_p(t) for t in out], _stream()), "usip_pair_augment")
+    return out
+
+
 def nms(keypoints, sigmas, radius):
     """keypoints (B,3,M) f32, sigmas (B,M) f32 -> (idx (B,M) i32 kept indices in emission order, -1 padded; count (B,) i32)."""
     _req(keypoints, f32, "keypoints"); _req(sigmas, f32, "sigmas")
