@@ -312,6 +312,17 @@ int usip_transform_points_bwd(const float* g_out, const float* R, const float* s
 
 /* ------------------------------------------------------------------------------------------------
  * 5. Backward pass of the fused plan (autograd of models/networks.py:75-162 / layers.py re-derived)
+ *
+ * Alignment: these kernels move 16-byte vectors, so the following operands must be 16-byte aligned (and their leading
+ * dimensions multiples of 4 floats); a misaligned one is rejected with -1 before any launch:
+ *   usip_bn_bwd_reduce      G, Y, scale, shift, mean, invstd, part
+ *   usip_bn_bwd_apply       G, Y, GY, scale, shift, mean, invstd, c1, c2
+ *   usip_groupmax_bwd_apply Y, gz, argsel, GY, scale, mean, invstd, c1, c2
+ *   usip_group_sum          G, out
+ *   usip_seg_sum            G, out
+ *   usip_head_bwd           G
+ *   usip_knn_combine_bwd    GY  (GZ may be unaligned or have ld % 4 != 0: it then takes scalar atomics)
+ * A column view at an offset that is not a multiple of 4 floats is therefore not accepted by these calls.
  * ---------------------------------------------------------------------------------------------- */
 /* train-mode BatchNorm(+ReLU) backward: partial sums of g_z and g_z*xhat per 128-row tile ([ntiles,2,C]) */
 int usip_bn_bwd_reduce(const float* G, int ldg, const float* Y, int ldy, const float* scale, const float* shift,

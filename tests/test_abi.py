@@ -47,6 +47,54 @@ int main(){ printf("%zu %zu %zu %zu %zu %zu\n", sizeof(usip_layer_desc), offseto
                    LayerDesc.gmax.offset, LayerDesc.precision.offset]
 
 
+def _misaligned_backward_calls():
+    """One call per (entry point, float4 operand) of the backward kernels with that operand 4 bytes off a 16-byte
+    boundary; every other pointer is aligned.  The addresses are never dereferenced: the argument check runs first."""
+    from usip_b200 import _lib
+    lib = _lib.load()
+    A = 0x100000
+
+    def ptrs(n, bad):
+        return [ctypes.c_void_p(A + 0x10000 * i + (4 if i == bad else 0)) for i in range(n)]
+
+    calls = []
+    for bad in range(7):      # G, Y, scale, shift, mean, invstd, part
+        G, Y, sc, sh, mu, iv, part = ptrs(7, bad)
+        calls.append(("bn_bwd_reduce", bad, lambda G=G, Y=Y, sc=sc, sh=sh, mu=mu, iv=iv, part=part:
+                      lib.usip_bn_bwd_reduce(G, 64, Y, 64, sc, sh, mu, iv, 1, part, 1000, 64, None)))
+        calls.append(("bn_bwd_reduce/C=48", bad, lambda G=G, Y=Y, sc=sc, sh=sh, mu=mu, iv=iv, part=part:
+                      lib.usip_bn_bwd_reduce(G, 48, Y, 48, sc, sh, mu, iv, 1, part, 1000, 48, None)))
+    for bad in range(9):      # G, Y, scale, shift, mean, invstd, c1, c2, GY
+        G, Y, sc, sh, mu, iv, c1, c2, GY = ptrs(9, bad)
+        for C in (64, 96):
+            calls.append(("bn_bwd_apply/C=%d" % C, bad, lambda G=G, Y=Y, sc=sc, sh=sh, mu=mu, iv=iv, c1=c1, c2=c2, GY=GY, C=C:
+                          lib.usip_bn_bwd_apply(G, C, Y, C, sc, sh, mu, iv, c1, c2, 1, GY, C, 1000, C, None)))
+    for bad in range(9):      # Y, gz, argsel, scale, mean, invstd, c1, c2, GY
+        Y, gz, a, sc, mu, iv, c1, c2, GY = ptrs(9, bad)
+        calls.append(("groupmax_bwd_apply", bad, lambda Y=Y, gz=gz, a=a, sc=sc, mu=mu, iv=iv, c1=c1, c2=c2, GY=GY:
+                      lib.usip_groupmax_bwd_apply(Y, 64, gz, a, sc, mu, iv, c1, c2, GY, 64, 16, 1600, 64, None)))
+    for bad in range(2):      # G, out
+        G, out = ptrs(2, bad)
+        calls.append(("group_sum", bad, lambda G=G, out=out: lib.usip_group_sum(G, 64, out, 64, 16, 100, 64, None)))
+        seg = ctypes.c_void_p(A + 0x80000)
+        calls.append(("seg_sum", bad, lambda G=G, out=out, seg=seg: lib.usip_seg_sum(G, 64, seg, out, 64, 2, 500, 8, 64, None)))
+    G, = ptrs(1, 0)
+    calls.append(("head_bwd", 0, lambda G=G: lib.usip_head_bwd(None, None, ctypes.c_void_p(A + 0x40000), 4, G, 2, 10, None)))
+    GY, = ptrs(1, 0)
+    aligned = ctypes.c_void_p(A + 0x40000)
+    calls.append(("knn_combine_bwd", 0, lambda GY=GY: lib.usip_knn_combine_bwd(GY, 128, aligned, aligned, aligned, 128, aligned,
+                                                                                128, 1, 32, 16, 128, None)))
+    return lib, calls
+
+
+def test_backward_entry_points_reject_misaligned_operands():
+    """A misaligned float4 operand is refused on the host (-1, no launch) -- it used to reach a kernel and fault the device."""
+    lib, calls = _misaligned_backward_calls()
+    for name, bad, fn in calls:
+        assert fn() == -1, (name, bad)
+        assert b"aligned" in lib.usip_last_error(), (name, bad, lib.usip_last_error())
+
+
 def test_product_path_fails_loudly_without_cuda():
     import torch
     if torch.cuda.is_available():

@@ -678,11 +678,13 @@ extern "C" int usip_bn_bwd_reduce(const float* G, int ldg, const float* Y, int l
   USIP_REQUIRE(G && Y && scale && shift && mean && invstd && part && C % 4 == 0 && ldg % 4 == 0 && ldy % 4 == 0 &&
                (C <= 128 ? (128 % C == 0 || C % 4 == 0) : C % 128 == 0), "bn_bwd_reduce: bad args");
   USIP_REQUIRE(C >= 32, "bn_bwd_reduce: C must be >= 32");
+  // both kernels read G, Y and the per-channel vectors as float4 (the fast one also writes part as float4)
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(part) |
+                 reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift) | reinterpret_cast<uintptr_t>(mean) |
+                 reinterpret_cast<uintptr_t>(invstd)) & 15) == 0,
+               "bn_bwd_reduce: operands must be 16-byte aligned");
   const int c4n = C / 4, ntiles = cdiv(P, BW_ROWS);
-  const bool aligned = ((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(part) |
-                         reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift) | reinterpret_cast<uintptr_t>(mean) |
-                         reinterpret_cast<uintptr_t>(invstd)) % 16) == 0;
-  if (aligned && c4n <= 256 && 256 % c4n == 0) {
+  if (c4n <= 256 && 256 % c4n == 0) {
     const int blocks = min(ntiles, device_sm_count() * 4);
     bn_bwd_reduce_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(G, ldg, Y, ldy, scale, shift, mean, invstd, relu, part, P, C, ntiles);
     return check_launch("bn_bwd_reduce_kernel");
@@ -703,13 +705,16 @@ extern "C" int usip_bn_bwd_finalize(const float* part, int ntiles, int64_t count
 extern "C" int usip_bn_bwd_apply(const float* G, int ldg, const float* Y, int ldy, const float* scale, const float* shift,
                                  const float* mean, const float* invstd, const float* c1, const float* c2, int relu,
                                  float* GY, int ldo, int P, int C, void* stream) {
-  USIP_REQUIRE(G && Y && GY && C % 4 == 0 && ldg % 4 == 0 && ldy % 4 == 0 && ldo % 4 == 0, "bn_bwd_apply: bad args");
+  USIP_REQUIRE(G && Y && GY && scale && shift && mean && invstd && c1 && c2 && C % 4 == 0 && ldg % 4 == 0 &&
+               ldy % 4 == 0 && ldo % 4 == 0, "bn_bwd_apply: bad args");
+  // G, Y, GY are float4 rows in both kernels; the fast one also reads the per-channel vectors as float4
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(GY) |
+                 reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift) | reinterpret_cast<uintptr_t>(mean) |
+                 reinterpret_cast<uintptr_t>(invstd) | reinterpret_cast<uintptr_t>(c1) | reinterpret_cast<uintptr_t>(c2)) & 15) == 0,
+               "bn_bwd_apply: operands must be 16-byte aligned");
   size_t total = (size_t)P * (C / 4);
   const int c4n = C / 4;
-  const bool aligned = ((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(GY) |
-                         reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift) | reinterpret_cast<uintptr_t>(mean) |
-                         reinterpret_cast<uintptr_t>(invstd) | reinterpret_cast<uintptr_t>(c1) | reinterpret_cast<uintptr_t>(c2)) % 16) == 0;
-  if (aligned && c4n <= 256 && 256 % c4n == 0) {
+  if (c4n <= 256 && 256 % c4n == 0) {
     const int rpp = 256 / c4n;
     const int blocks = (int)min((long long)device_sm_count() * 8, (long long)cdiv(P, rpp * 4));
     bn_bwd_apply_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(G, ldg, Y, ldy, scale, shift, mean, invstd, c1, c2, relu, GY, ldo, P, C);
@@ -744,9 +749,10 @@ extern "C" int usip_groupmax_bwd_apply(const float* Y, int ldy, const float* gz,
                                        const float* scale, const float* mean, const float* invstd, const float* c1,
                                        const float* c2, float* GY, int ldo, int K, int P, int C, void* stream) {
   USIP_REQUIRE(Y && gz && argsel && GY && C % 4 == 0 && ldy % 4 == 0 && ldo % 4 == 0, "groupmax_bwd_apply: bad args");
-  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(mean) | reinterpret_cast<uintptr_t>(invstd) |
-                 reinterpret_cast<uintptr_t>(c1) | reinterpret_cast<uintptr_t>(c2)) & 15) == 0,
-               "groupmax_bwd_apply: per-channel vectors must be 16-byte aligned");
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(gz) | reinterpret_cast<uintptr_t>(argsel) |
+                 reinterpret_cast<uintptr_t>(GY) | reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(mean) |
+                 reinterpret_cast<uintptr_t>(invstd) | reinterpret_cast<uintptr_t>(c1) | reinterpret_cast<uintptr_t>(c2)) & 15) == 0,
+               "groupmax_bwd_apply: operands must be 16-byte aligned");
   size_t total = (size_t)P * (C / 4);
   int blocks = (int)min((size_t)device_sm_count() * 16, cdiv64(total, 256));
   groupmax_bwd_apply_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(Y, ldy, gz, argsel, scale, mean, invstd, c1, c2, GY,
@@ -756,6 +762,8 @@ extern "C" int usip_groupmax_bwd_apply(const float* Y, int ldy, const float* gz,
 
 extern "C" int usip_group_sum(const float* G, int ldg, float* out, int ldo, int K, int Q, int C, void* stream) {
   USIP_REQUIRE(G && out && C % 4 == 0 && ldg % 4 == 0 && ldo % 4 == 0, "group_sum: bad args");
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+               "group_sum: G and out must be 16-byte aligned");
   size_t n = (size_t)Q * (C / 4);
   group_sum_kernel<<<(unsigned)cdiv64(n, 256), 256, 0, (cudaStream_t)stream>>>(G, ldg, out, ldo, K, Q, C);
   return check_launch("group_sum_kernel");
@@ -764,6 +772,8 @@ extern "C" int usip_group_sum(const float* G, int ldg, float* out, int ldo, int 
 extern "C" int usip_seg_sum(const float* G, int ldg, const int32_t* seg_off, float* out, int ldo, int B, int N, int M,
                             int C, void* stream) {
   USIP_REQUIRE(G && seg_off && out && C % 4 == 0 && ldg % 4 == 0 && ldo % 4 == 0, "seg_sum: bad args");
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+               "seg_sum: G and out must be 16-byte aligned");
   seg_sum_kernel<<<cdiv(B * M * 32, 256), 256, 0, (cudaStream_t)stream>>>(G, ldg, seg_off, out, ldo, B, N, M, C);
   return check_launch("seg_sum_kernel");
 }
@@ -779,6 +789,7 @@ extern "C" int usip_unpool_scatter(float* G, int ldg, const float* gp, int ldp, 
 extern "C" int usip_knn_combine_bwd(const float* GY, int ldg, const float* pts, const int32_t* knn_idx, float* GZ,
                                     int ldz, float* gW, int ldw, int B, int M, int K, int C, void* stream) {
   USIP_REQUIRE(GY && pts && knn_idx && GZ && gW && C % 4 == 0 && ldg % 4 == 0, "knn_combine_bwd: bad args");
+  USIP_REQUIRE((reinterpret_cast<uintptr_t>(GY) & 15) == 0, "knn_combine_bwd: GY must be 16-byte aligned");
   int G = B * M * K;
   knn_combine_bwd_kernel<<<cdiv(G, BW_ROWS), 256, (size_t)C * 3 * sizeof(float), (cudaStream_t)stream>>>(
       GY, ldg, pts, knn_idx, GZ, ldz, gW, ldw, B, M, K, C);
@@ -801,6 +812,7 @@ extern "C" int usip_colsum(const float* G, int ldg, float* out, int P, int C, vo
 extern "C" int usip_head_bwd(const float* g_kp, const float* g_sig, const float* out4, int ld, float* G, int B, int M,
                              void* stream) {
   USIP_REQUIRE(out4 && G, "head_bwd: bad args");
+  USIP_REQUIRE((reinterpret_cast<uintptr_t>(G) & 15) == 0, "head_bwd: G must be 16-byte aligned");
   head_bwd_kernel<<<cdiv(B * M, 256), 256, 0, (cudaStream_t)stream>>>(g_kp, g_sig, out4, ld, G, B, M);
   return check_launch("head_bwd_kernel");
 }

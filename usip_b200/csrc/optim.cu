@@ -5,8 +5,12 @@
 // one launch over the flat parameter / gradient / moment buffers the host side keeps (usip_b200/optim.py).  The step
 // counter and the learning rate live in DEVICE memory so that the launch can sit inside a CUDA graph: the kernel reads
 // step t-1, updates with the bias corrections of step t, and the last CTA to arrive publishes t.
-// Arithmetic follows torch's single-tensor Adam: m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;
-// p -= (lr / (1-b1^t)) * m / (sqrt(v) / sqrt(1-b2^t) + eps).
+// The update is torch's Adam in fp32, m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;
+// p -= (lr / (1-b1^t)) * m / (sqrt(v) / sqrt(1-b2^t) + eps), but not its exact rounding: torch's single-tensor path
+// updates m as a lerp, m + (1-b1)(g - m), and divides by sqrt(1-b2^t), where this kernel forms b1 m + (1-b1) g and
+// multiplies by a (double-rounded) 1/sqrt(1-b2^t).  The betas arrive as float, so the moments decay with the fp32 betas
+// (1 - 0.999f is 1.3e-5 below 0.001, so v is 1.3e-5 below torch's); the bias corrections use the same betas, which
+// cancels that difference in the update.
 #include "common.cuh"
 
 namespace usip {
@@ -27,7 +31,7 @@ adam_step_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
     float mv[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w}, pv[4] = {p4.x, p4.y, p4.z, p4.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      mv[j] = __fadd_rn(__fmul_rn(mv[j], beta1), __fmul_rn(gv[j], omb1));                 // lerp as torch: m + (g-m)(1-b1)
+      mv[j] = __fadd_rn(__fmul_rn(mv[j], beta1), __fmul_rn(gv[j], omb1));                 // b1 m + (1-b1) g (not torch's lerp)
       vv[j] = __fadd_rn(__fmul_rn(vv[j], beta2), __fmul_rn(__fmul_rn(gv[j], gv[j]), omb2));
       const float denom = __fadd_rn(__fmul_rn(sqrtf(vv[j]), inv_bc2_sqrt), eps);
       pv[j] = __fsub_rn(pv[j], __fmul_rn(step_size, __fdiv_rn(mv[j], denom)));
