@@ -118,6 +118,34 @@ int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const i
                       int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node, float* dst_pc,
                       float* dst_sn, float* dst_node, float* R, float* scale, float* shift, void* stream);
 
+/* Descriptor training pairs on the device (csrc/pairgen.cu)  data/kitti_descriptor_loader.py:102-347
+ * (KittiDescriptorLoader.__getitem__).  Same scans / offsets / clouds as above, but the anchor (side 0) and the positive
+ * (side 1) of a pair are different scans: scan_of_cloud (2*n_pairs) i32 names the scan of every cloud.  The Philox keys
+ * are those of the detector calls for the same cloud number.
+ *
+ * usip_cloud_subsample (get_instance_unaugmented_np, :117-128): out_rows (2*n_pairs, N) i32, a uniform subset of N
+ *   rows without replacement, ascending; out_cand (2*n_pairs, n_cand) i32 and out_start (2*n_pairs) i32 as in
+ *   usip_pair_subsample.  No radius mask.  Every scan must hold at least N rows (the reference raises otherwise; the
+ *   callers reject such scans); max_rows and the limit as in usip_pair_subsample.
+ * usip_cloud_gather_candidates: out_pts (2*n_pairs, n_cand, 3) f32 = xyz of rows[c, cand[c, j]] of scan_of_cloud[c].
+ * usip_desc_pair_augment (augment(), :205-276, train mode only):
+ *   params (2*n_pairs, 32) f64 per cloud: [0:9] horizontal, [9:18] 3-d and [18:27] perturbation rotation matrices
+ *     (row major, data @ R in float64), [28:31] the shift; [27] unused;  scale (n_pairs) f64 per pair;
+ *   jitter arrays and flags as in usip_pair_augment (the transform flags only); sn = columns 3:3+S for every S
+ *     (3 + S <= C).  Test mode (no USIP_PAIR_TRAIN): the rows and the nodes as they are.
+ *   -> anc/pos pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M) f32. */
+int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud, int max_rows,
+                         int n_pairs, int N, int n_cand, uint64_t seed, uint64_t step, int32_t* out_rows,
+                         int32_t* out_cand, int32_t* out_start, void* stream);
+int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                                 const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
+                                 int n_cand, void* stream);
+int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                           const int32_t* rows, const float* nodes, const double* params, const double* scale,
+                           const double* jit_pc, const double* jit_sn, const double* jit_node, uint64_t seed,
+                           uint64_t step, int flags, int S, int n_pairs, int N, int M, float* anc_pc, float* anc_sn,
+                           float* anc_node, float* pos_pc, float* pos_sn, float* pos_node, void* stream);
+
 /* Radius non-maximum suppression of the detected keypoints    evaluation/save_keypoints.py:180-216 (nms)
  * keypoints (B,3,M) f32, sigmas (B,M) f32 -> out_idx (B,M) i32: original indices of the kept keypoints in the order the
  * reference emits them (ascending sigma, ties by index), padded with -1; out_count (B,) i32.  radius < 0.01: pass-through

@@ -360,6 +360,70 @@ def golden_pairs(ref):
     np.savez_compressed(os.path.join(OUT, "detector_pairs.npz"), **out)
 
 
+# data/kitti_descriptor_loader.py KittiDescriptorLoader.__getitem__ + mine_negative_sample on a synthetic KITTI tree with
+# a pose trajectory: sequence 0 is 40 scans 1.5 m apart along a gently turning path (positives within 5 m, scans more
+# than 50 m apart), the other sequences a few scans each.  Every scan is (DESC_NS, 8) float32.
+DESC_COUNTS = [40, 3, 2, 2, 2, 2, 2, 2, 3, 3, 3]
+DESC_NS, DESC_TREE_SEED, DESC_N, DESC_M = 700, 7200, 512, 32
+DESC_CASES = {     # name: (mode, anchors, np/random seed, S, rot_horizontal, rot_3d, rot_perturbation, translation)
+    "kitti": ("train", [3, 41, 17, 44], 21, 4, 1, 0, 0, 0),
+    "s1": ("train", [40, 7, 52, 30], 22, 1, 1, 0, 0, 0),
+    "s5": ("train", [22, 5, 20, 39], 23, 5, 1, 0, 0, 0),       # anchors 0 and 2 have no negative in this batch
+    "rot3d": ("train", [12, 45, 48, 0], 24, 3, 0, 1, 1, 1),
+    "test": ("test", [0, 4, 2, 5], 25, 4, 1, 0, 0, 0),
+}
+
+
+def desc_trajectory(counts):
+    """poses[seq][i] (4, 4) float64: sequence s runs along a heading that turns 1 degree per scan, 1.5 m per scan,
+    from an offset of 1000 m * s."""
+    poses = []
+    for s, n in enumerate(counts):
+        ps, pos, yaw = [], np.array([1000.0 * s, 0.0, 0.0]), 0.3 * s
+        for i in range(n):
+            c, si = np.cos(yaw), np.sin(yaw)
+            P = np.eye(4)
+            P[:3, :3] = [[c, 0, si], [0, 1, 0], [-si, 0, c]]
+            P[:3, 3] = pos
+            ps.append(P)
+            pos = pos + 1.5 * np.array([si, 0.0, c])
+            yaw += np.pi / 180
+        poses.append(ps)
+    return poses
+
+
+def golden_descpairs(ref):
+    import importlib
+    import tempfile
+    from torch.utils.data.dataloader import default_collate
+    from usip_b200.data.kitti_detector_loader import write_synthetic_kitti
+    kl = importlib.import_module("data.kitti_descriptor_loader")
+    poses = desc_trajectory(DESC_COUNTS)
+    out = {"tree/counts": np.array(DESC_COUNTS), "tree/Ns": np.int64(DESC_NS), "tree/seed": np.int64(DESC_TREE_SEED),
+           "tree/poses": np.concatenate([np.stack(p) for p in poses if p]), "N": np.int64(DESC_N), "M": np.int64(DESC_M)}
+    keys = ("anc_pc", "anc_sn", "anc_node", "anc_seq", "anc_pose", "pos_pc", "pos_sn", "pos_node", "pos_seq", "pos_pose")
+    with tempfile.TemporaryDirectory() as root:
+        write_synthetic_kitti(root, DESC_COUNTS, DESC_NS, seed=DESC_TREE_SEED, poses=poses)
+        for name, (mode, anchors, seed, S, rh, r3, rp, tp) in DESC_CASES.items():
+            opt = ref_shim.make_opt(input_pc_num=DESC_N, node_num=DESC_M, surface_normal_len=S, rot_horizontal=bool(rh),
+                                    rot_3d=bool(r3), rot_perturbation=bool(rp), translation_perturbation=bool(tp),
+                                    positive_radius_threshold=5.0, negative_radius_threshold=50.0)
+            loader = kl.KittiDescriptorLoader(root, mode, opt)
+            np.random.seed(seed)
+            random.seed(seed)
+            batch = default_collate([loader[i] for i in anchors])
+            neg_idx = loader.mine_negative_sample(batch[3], batch[4], opt.negative_radius_threshold)
+            out[name + "/case"] = np.array([seed, S, rh, r3, rp, tp], dtype=np.int64)
+            out[name + "/anchors"] = np.array(anchors, dtype=np.int64)
+            out[name + "/mode"] = np.array(mode)
+            for k, v in zip(keys, batch):
+                out[name + "/" + k] = v.numpy()
+            out[name + "/neg_idx"] = neg_idx.numpy()
+            print("descpairs", name, "pos_seq", out[name + "/pos_seq"], "neg_idx", out[name + "/neg_idx"])
+    np.savez_compressed(os.path.join(OUT, "descriptor_pairs.npz"), **out)
+    print("descriptor_pairs.npz", os.path.getsize(os.path.join(OUT, "descriptor_pairs.npz")) // 1024, "KB")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)

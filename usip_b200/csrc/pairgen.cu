@@ -7,7 +7,12 @@
 // stream: the index lists and jitter arrays) or generated here with Philox4x32-10 keyed by (seed, step, cloud, point,
 // purpose), so that a batch is a pure function of (seed, step).
 //
-// Clouds are numbered c = 2*pair + side (side 0 = src, 1 = dst); both sides of a pair come from the same scan.
+// Clouds are numbered c = 2*pair + side (side 0 = src / anchor, 1 = dst / positive).  The subset and gather kernels read
+// the scan of cloud c as scan_of[c >> pair_shift]: pair_shift = 1 for the detector (both sides of a pair subsample the
+// same scan), 0 for the descriptor (the anchor and the positive are different scans).  The Philox counters depend on c
+// only, so the mapping changes no random number.
+#include <stdio.h>
+
 #include "common.cuh"
 
 namespace usip {
@@ -16,6 +21,7 @@ constexpr int PG_THREADS = 1024;                   // subset kernel: one CTA per
 constexpr int PG_AUG_THREADS = 256;
 constexpr uint32_t PG_SENTINEL = 0xffffffffu;      // key of a point that may not be drawn (outside the radius)
 constexpr int PG_PARAM_STRIDE = 48;                // doubles per pair, see usip_pair_augment in the header
+constexpr int PG_DESC_PARAM_STRIDE = 32;           // doubles per cloud, see usip_desc_pair_augment in the header
 
 enum { PURPOSE_ROWS = 0, PURPOSE_CAND = 1, PURPOSE_START = 2, PURPOSE_JIT_PC = 3, PURPOSE_JIT_SN = 4,
        PURPOSE_JIT_NODE = 5 };
@@ -130,7 +136,8 @@ __device__ __forceinline__ bool pg_inside(const float* p, double radius) {
 // level 1: the N/3 FPS candidates as ascending positions into the rows, and the FPS start index.
 __global__ void __launch_bounds__(PG_THREADS)
 pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
-                   const int32_t* __restrict__ scan_of_cloud, int level, int use_radius, double radius, int N, int n_cand,
+                   const int32_t* __restrict__ scan_of, int pair_shift, int level, int use_radius, double radius, int N,
+                   int n_cand,
                    uint64_t seed, uint64_t step, int32_t* __restrict__ out_rows, int32_t* __restrict__ out_cand,
                    int32_t* __restrict__ out_start, int32_t* __restrict__ out_valid) {
   extern __shared__ __align__(16) unsigned char pg_smem[];
@@ -139,7 +146,7 @@ pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __rest
   __shared__ uint64_t s_warp[32];
   uint32_t* key = reinterpret_cast<uint32_t*>(pg_smem);
   const int c = blockIdx.x, tid = threadIdx.x;
-  const int scan = scan_of_cloud[c / 2];
+  const int scan = scan_of[c >> pair_shift];
   const int64_t row0 = offsets[scan];
   const int n = level == 0 ? (int)(offsets[scan + 1] - row0) : N;
   const float* base = scans + row0 * C;
@@ -207,12 +214,12 @@ pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __rest
 
 // candidate points for FPS: pts[c, j, :] = xyz of row rows[c, cand[c, j]]
 __global__ void pair_gather_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
-                                   const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
+                                   const int32_t* __restrict__ scan_of, int pair_shift, const int32_t* __restrict__ rows,
                                    const int32_t* __restrict__ cand, float* __restrict__ pts, int N, int n_cand) {
   const int c = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n_cand) return;
   const int r = rows[(int64_t)c * N + cand[(int64_t)c * n_cand + j]];
-  const float* p = scans + (offsets[scan_of_cloud[c / 2]] + r) * C;
+  const float* p = scans + (offsets[scan_of[c >> pair_shift]] + r) * C;
   float* o = pts + ((int64_t)c * n_cand + j) * 3;
   o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
 }
@@ -237,6 +244,93 @@ __device__ __forceinline__ void pg_colvec(float& x, float& y, float& z, const fl
 
 constexpr int PG_MAX_S = 8;
 
+// --------------------------------------------------------------- train-time augmentation shared by both loaders
+// kitti_detector_loader.py:182-212 (KittiLoader.augment) and kitti_descriptor_loader.py:240-272
+// (KittiDescriptorLoader.augment) apply the same arithmetic to every cloud; these helpers are that arithmetic, so the
+// two kernels cannot drift apart.  P points at one cloud's [0:27] rotation matrices (horizontal, 3-d, perturbation)
+// and [28:31] shift; sc is the augmentation scale; flags the USIP_PAIR_* bits.
+// Flags: USIP_PAIR_ROT_HORIZONTAL << r is rotation r.
+constexpr int PG_ANY_ROT = USIP_PAIR_ROT_HORIZONTAL | USIP_PAIR_ROT_3D | USIP_PAIR_ROT_PERTURBATION;
+
+// clipped N(0, 0.04^2) jitter of one point or node (pc and nodes use the same law): uploaded, or Philox
+__device__ __forceinline__ void pg_jitter_xyz(const double* jit, int64_t at, uint64_t seed, uint64_t step, int c, int i,
+                                              int purpose, double j[4]) {
+  if (jit) {
+    const double* q = jit + at * 3;
+    j[0] = q[0]; j[1] = q[1]; j[2] = q[2];
+  } else {
+    const uint4 u = pg_random(seed, step, c, i, purpose, 0);
+    pg_normal2(u.x, u.y, j[0], j[1]); pg_normal2(u.z, u.w, j[2], j[3]);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) j[k] = pg_clip(0.04 * j[k], 0.12);
+  }
+}
+
+// one point: rotations (pc in float64, sn a float32 view rounded after every rotation), jitter, scale, shift
+__device__ __forceinline__ void pg_augment_point(int flags, const double* P, double sc, const double* j, int S,
+                                                 float& x, float& y, float& z, float* sn) {
+  double X = x, Y = y, Z = z;
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    if (!(flags & (USIP_PAIR_ROT_HORIZONTAL << r))) continue;
+    pg_rowvec(X, Y, Z, P + 9 * r);
+    if (S >= 3) {
+      double a = sn[0], bb = sn[1], cc = sn[2];
+      pg_rowvec(a, bb, cc, P + 9 * r);
+      sn[0] = (float)a; sn[1] = (float)bb; sn[2] = (float)cc;
+    }
+  }
+  if (flags & PG_ANY_ROT) {                                 // pc is float64 after the first rotation
+    X = __dadd_rn(X, j[0]); Y = __dadd_rn(Y, j[1]); Z = __dadd_rn(Z, j[2]);
+    X = __dmul_rn(X, sc); Y = __dmul_rn(Y, sc); Z = __dmul_rn(Z, sc);
+    if (flags & USIP_PAIR_TRANSLATION) { X = __dadd_rn(X, P[28]); Y = __dadd_rn(Y, P[29]); Z = __dadd_rn(Z, P[30]); }
+    x = (float)X; y = (float)Y; z = (float)Z;
+  } else {                                         // pc is still the float32 slice: every step rounds to fp32
+    x = (float)__dadd_rn((double)x, j[0]); y = (float)__dadd_rn((double)y, j[1]);
+    z = (float)__dadd_rn((double)z, j[2]);
+    const float scf = (float)sc;                   // float32 array * Python float
+    x = __fmul_rn(x, scf); y = __fmul_rn(y, scf); z = __fmul_rn(z, scf);
+    if (flags & USIP_PAIR_TRANSLATION) {
+      x = (float)__dadd_rn((double)x, P[28]); y = (float)__dadd_rn((double)y, P[29]);
+      z = (float)__dadd_rn((double)z, P[30]);
+    }
+  }
+}
+
+// sn jitter: fl32(double(sn) + j) with j clipped N(0, 0.01^2), never scaled or shifted; at = the point's row in jit_sn
+__device__ __forceinline__ void pg_jitter_sn(const double* jit_sn, int64_t at, uint64_t seed, uint64_t step, int c,
+                                             int i, int S, float* sn) {
+#pragma unroll
+  for (int q = 0; q < PG_MAX_S; q += 4) {
+    if (q >= S) break;
+    double js[4];
+    if (jit_sn) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) js[k] = q + k < S ? jit_sn[at * S + q + k] : 0.0;
+    } else {
+      const uint4 u = pg_random(seed, step, c, i, PURPOSE_JIT_SN, q / 4);
+      pg_normal2(u.x, u.y, js[0], js[1]); pg_normal2(u.z, u.w, js[2], js[3]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) js[k] = pg_clip(0.01 * js[k], 0.05);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (q + k < S) sn[q + k] = (float)__dadd_rn((double)sn[q + k], js[k]);
+  }
+}
+
+// one node: float64 (FarthestSampler output) through rotations, jitter, scale and shift until the final cast
+__device__ __forceinline__ void pg_augment_node(int flags, const double* P, double sc, const double* j, float& x,
+                                                float& y, float& z) {
+  double X = x, Y = y, Z = z;
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    if (flags & (USIP_PAIR_ROT_HORIZONTAL << r)) pg_rowvec(X, Y, Z, P + 9 * r);
+  X = __dmul_rn(__dadd_rn(X, j[0]), sc); Y = __dmul_rn(__dadd_rn(Y, j[1]), sc); Z = __dmul_rn(__dadd_rn(Z, j[2]), sc);
+  if (flags & USIP_PAIR_TRANSLATION) { X = __dadd_rn(X, P[28]); Y = __dadd_rn(Y, P[29]); Z = __dadd_rn(Z, P[30]); }
+  x = (float)X; y = (float)Y; z = (float)Z;
+}
+
 __global__ void __launch_bounds__(PG_AUG_THREADS)
 pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
                     const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
@@ -250,10 +344,6 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const double* P = params + (int64_t)b * PG_PARAM_STRIDE;
   const bool train = flags & USIP_PAIR_TRAIN;
-  const bool rot[3] = {(flags & USIP_PAIR_ROT_HORIZONTAL) != 0, (flags & USIP_PAIR_ROT_3D) != 0,
-                       (flags & USIP_PAIR_ROT_PERTURBATION) != 0};
-  const bool any_rot = rot[0] || rot[1] || rot[2];
-  const bool translate = flags & USIP_PAIR_TRANSLATION;
   float RT[9];
 #pragma unroll
   for (int k = 0; k < 9; ++k) RT[k] = (float)P[31 + k];
@@ -272,61 +362,10 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
 #pragma unroll
     for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[sn_col + k] : 0.f;
     if (train) {                                   // KittiLoader.augment, :182-212
-      double X = x, Y = y, Z = z;
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-        if (!rot[r]) continue;
-        pg_rowvec(X, Y, Z, P + 9 * r);
-        if (S >= 3) {                              // sn is a float32 view: rounded after every rotation
-          double a = sn[0], bb = sn[1], cc = sn[2];
-          pg_rowvec(a, bb, cc, P + 9 * r);
-          sn[0] = (float)a; sn[1] = (float)bb; sn[2] = (float)cc;
-        }
-      }
       double j[4];
-      if (jit_pc) {
-        const double* q = jit_pc + ((int64_t)c * N + i) * 3;
-        j[0] = q[0]; j[1] = q[1]; j[2] = q[2];
-      } else {
-        const uint4 u = pg_random(seed, step, c, i, PURPOSE_JIT_PC, 0);
-        pg_normal2(u.x, u.y, j[0], j[1]); pg_normal2(u.z, u.w, j[2], j[3]);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) j[k] = pg_clip(0.04 * j[k], 0.12);
-      }
-      const double sc = P[27];
-      if (any_rot) {                               // pc is float64 after the first rotation
-        X = __dadd_rn(X, j[0]); Y = __dadd_rn(Y, j[1]); Z = __dadd_rn(Z, j[2]);
-        X = __dmul_rn(X, sc); Y = __dmul_rn(Y, sc); Z = __dmul_rn(Z, sc);
-        if (translate) { X = __dadd_rn(X, P[28]); Y = __dadd_rn(Y, P[29]); Z = __dadd_rn(Z, P[30]); }
-        x = (float)X; y = (float)Y; z = (float)Z;
-      } else {                                     // pc is still the float32 slice: every step rounds to fp32
-        x = (float)__dadd_rn((double)x, j[0]); y = (float)__dadd_rn((double)y, j[1]);
-        z = (float)__dadd_rn((double)z, j[2]);
-        const float scf = (float)sc;               // float32 array * Python float
-        x = __fmul_rn(x, scf); y = __fmul_rn(y, scf); z = __fmul_rn(z, scf);
-        if (translate) {
-          x = (float)__dadd_rn((double)x, P[28]); y = (float)__dadd_rn((double)y, P[29]);
-          z = (float)__dadd_rn((double)z, P[30]);
-        }
-      }
-      // sn jitter: fl32(double(sn) + j), never scaled or shifted
-#pragma unroll
-      for (int q = 0; q < PG_MAX_S; q += 4) {
-        if (q >= S) break;
-        double js[4];
-        if (jit_sn) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) js[k] = q + k < S ? jit_sn[((int64_t)c * N + i) * S + q + k] : 0.0;
-        } else {
-          const uint4 u = pg_random(seed, step, c, i, PURPOSE_JIT_SN, q / 4);
-          pg_normal2(u.x, u.y, js[0], js[1]); pg_normal2(u.z, u.w, js[2], js[3]);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) js[k] = pg_clip(0.01 * js[k], 0.05);
-        }
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          if (q + k < S) sn[q + k] = (float)__dadd_rn((double)sn[q + k], js[k]);
-      }
+      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, j);
+      pg_augment_point(flags, P, P[27], j, S, x, y, z, sn);
+      pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, sn);
     }
     float* opc = side ? dst_pc : src_pc;
     float* osn = side ? dst_sn : src_sn;
@@ -345,28 +384,13 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
       if (k < S) osn[((int64_t)b * S + k) * N + i] = sn[k];
   }
 
-  if (i < M) {                                     // nodes: float64 (FarthestSampler output) until the final cast
+  if (i < M) {
     const float* nd = nodes + (int64_t)c * 3 * M;
     float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
     if (train) {
-      double X = x, Y = y, Z = z;
-#pragma unroll
-      for (int r = 0; r < 3; ++r)
-        if (rot[r]) pg_rowvec(X, Y, Z, P + 9 * r);
       double j[4];
-      if (jit_node) {
-        const double* q = jit_node + ((int64_t)c * M + i) * 3;
-        j[0] = q[0]; j[1] = q[1]; j[2] = q[2];
-      } else {
-        const uint4 u = pg_random(seed, step, c, i, PURPOSE_JIT_NODE, 0);
-        pg_normal2(u.x, u.y, j[0], j[1]); pg_normal2(u.z, u.w, j[2], j[3]);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) j[k] = pg_clip(0.04 * j[k], 0.12);
-      }
-      const double sc = P[27];
-      X = __dmul_rn(__dadd_rn(X, j[0]), sc); Y = __dmul_rn(__dadd_rn(Y, j[1]), sc); Z = __dmul_rn(__dadd_rn(Z, j[2]), sc);
-      if (translate) { X = __dadd_rn(X, P[28]); Y = __dadd_rn(Y, P[29]); Z = __dadd_rn(Z, P[30]); }
-      x = (float)X; y = (float)Y; z = (float)Z;
+      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, j);
+      pg_augment_node(flags, P, P[27], j, x, y, z);
     }
     float* ond = side ? dst_node : src_node;
     if (side == 1) {
@@ -375,6 +399,59 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
       x = __fmul_rn(x, sc); y = __fmul_rn(y, sc); z = __fmul_rn(z, sc);
       x = __fadd_rn(x, (float)P[40]); y = __fadd_rn(y, (float)P[41]); z = __fadd_rn(z, (float)P[42]);
     }
+    ond[((int64_t)b * 3 + 0) * M + i] = x;
+    ond[((int64_t)b * 3 + 1) * M + i] = y;
+    ond[((int64_t)b * 3 + 2) * M + i] = z;
+  }
+}
+
+// Descriptor pairs (KittiDescriptorLoader.augment, kitti_descriptor_loader.py:205-276): every cloud has its own scan,
+// rotations, jitter and shift; the scale is the pair's.  No dst transform.  sn = columns 3:3+S for every S.
+__global__ void __launch_bounds__(PG_AUG_THREADS)
+desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
+                         const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
+                         const float* __restrict__ nodes, const double* __restrict__ params,
+                         const double* __restrict__ scale, const double* __restrict__ jit_pc,
+                         const double* __restrict__ jit_sn, const double* __restrict__ jit_node, uint64_t seed,
+                         uint64_t step, int flags, int S, int N, int M, float* __restrict__ anc_pc,
+                         float* __restrict__ anc_sn, float* __restrict__ anc_node, float* __restrict__ pos_pc,
+                         float* __restrict__ pos_sn, float* __restrict__ pos_node) {
+  const int c = blockIdx.y, b = c >> 1, side = c & 1;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const double* P = params + (int64_t)c * PG_DESC_PARAM_STRIDE;
+  const bool train = flags & USIP_PAIR_TRAIN;
+
+  if (i < N) {
+    const float* p = scans + (offsets[scan_of_cloud[c]] + rows[(int64_t)c * N + i]) * C;
+    float x = p[0], y = p[1], z = p[2];
+    float sn[PG_MAX_S];
+#pragma unroll
+    for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[3 + k] : 0.f;
+    if (train) {
+      double j[4];
+      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, j);
+      pg_augment_point(flags, P, scale[b], j, S, x, y, z, sn);
+      pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, sn);
+    }
+    float* opc = side ? pos_pc : anc_pc;
+    float* osn = side ? pos_sn : anc_sn;
+    opc[((int64_t)b * 3 + 0) * N + i] = x;
+    opc[((int64_t)b * 3 + 1) * N + i] = y;
+    opc[((int64_t)b * 3 + 2) * N + i] = z;
+#pragma unroll
+    for (int k = 0; k < PG_MAX_S; ++k)
+      if (k < S) osn[((int64_t)b * S + k) * N + i] = sn[k];
+  }
+
+  if (i < M) {
+    const float* nd = nodes + (int64_t)c * 3 * M;
+    float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
+    if (train) {
+      double j[4];
+      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, j);
+      pg_augment_node(flags, P, scale[b], j, x, y, z);
+    }
+    float* ond = side ? pos_node : anc_node;
     ond[((int64_t)b * 3 + 0) * M + i] = x;
     ond[((int64_t)b * 3 + 1) * M + i] = y;
     ond[((int64_t)b * 3 + 2) * M + i] = z;
@@ -391,37 +468,93 @@ extern "C" int usip_pair_max_scan_rows(void) {
   return (227 * 1024 - 4096) / (int)sizeof(uint32_t);
 }
 
+// "<entry point>: <reason>" as the last error
+static int pg_fail(const char* what, const char* why) {
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", what, why);
+  set_last_error(msg);
+  return -1;
+}
+#define PG_REQUIRE(cond, why) do { if (!(cond)) return pg_fail(what, why); } while (0)
+
+// rows, then candidates + FPS start, of 2*n_pairs clouds (see the cloud -> scan mapping at the top)
+static int pg_subsample(const char* what, const float* scans, int C, const int64_t* offsets, const int32_t* scan_of,
+                        int pair_shift, int max_rows, int n_pairs, int N, int n_cand, int use_radius, double radius,
+                        uint64_t seed, uint64_t step, int32_t* out_rows, int32_t* out_cand, int32_t* out_start,
+                        int32_t* out_valid, void* stream) {
+  PG_REQUIRE(scans && offsets && scan_of && out_rows && out_cand && out_start, "null pointer");
+  PG_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N && max_rows > 0, "bad sizes");
+  const int smem = pg_subset_smem(max(max_rows, N));
+  PG_REQUIRE(max(max_rows, N) <= usip_pair_max_scan_rows(), "scan or N too large for shared memory");
+  cudaError_t e = cudaFuncSetAttribute(pair_subset_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) { pg_fail(what, "smem attribute"); return (int)e; }
+  cudaStream_t s = (cudaStream_t)stream;
+  pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(max_rows), s>>>(
+      scans, C, offsets, scan_of, pair_shift, 0, use_radius, radius, N, n_cand, seed, step, out_rows, out_cand,
+      out_start, out_valid);
+  int rc = check_launch("pair_subset_kernel(rows)");
+  if (rc) return rc;
+  pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(N), s>>>(
+      scans, C, offsets, scan_of, pair_shift, 1, 0, 0.0, N, n_cand, seed, step, out_rows, out_cand, out_start,
+      out_valid);
+  return check_launch("pair_subset_kernel(candidates)");
+}
+
+static int pg_gather(const char* what, const float* scans, int C, const int64_t* offsets, const int32_t* scan_of,
+                     int pair_shift, const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
+                     int n_cand, void* stream) {
+  PG_REQUIRE(scans && offsets && scan_of && rows && cand && out_pts, "null pointer");
+  PG_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N, "bad sizes");
+  dim3 grid(cdiv(n_cand, 256), 2 * n_pairs);
+  pair_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of, pair_shift, rows, cand,
+                                                              out_pts, N, n_cand);
+  return check_launch("pair_gather_kernel");
+}
+
 extern "C" int usip_pair_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,
                                    int max_rows, int n_pairs, int N, int n_cand, int use_radius, double radius,
                                    uint64_t seed, uint64_t step, int32_t* out_rows, int32_t* out_cand,
                                    int32_t* out_start, int32_t* out_valid, void* stream) {
-  USIP_REQUIRE(scans && offsets && scan_of_pair && out_rows && out_cand && out_start, "pair_subsample: null pointer");
-  USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N && max_rows > 0,
-               "pair_subsample: bad sizes");
-  const int smem = pg_subset_smem(max(max_rows, N));
-  USIP_REQUIRE(max(max_rows, N) <= usip_pair_max_scan_rows(), "pair_subsample: scan or N too large for shared memory");
-  cudaError_t e = cudaFuncSetAttribute(pair_subset_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (e != cudaSuccess) { set_last_error("pair_subsample: smem attribute"); return (int)e; }
-  cudaStream_t s = (cudaStream_t)stream;
-  pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(max_rows), s>>>(
-      scans, C, offsets, scan_of_pair, 0, use_radius, radius, N, n_cand, seed, step, out_rows, out_cand, out_start,
-      out_valid);
-  int rc = check_launch("pair_subset_kernel(rows)");
-  if (rc) return rc;
-  pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(N), s>>>(
-      scans, C, offsets, scan_of_pair, 1, 0, 0.0, N, n_cand, seed, step, out_rows, out_cand, out_start, out_valid);
-  return check_launch("pair_subset_kernel(candidates)");
+  return pg_subsample("pair_subsample", scans, C, offsets, scan_of_pair, 1, max_rows, n_pairs, N, n_cand, use_radius,
+                      radius, seed, step, out_rows, out_cand, out_start, out_valid, stream);
 }
 
 extern "C" int usip_pair_gather_candidates(const float* scans, int C, const int64_t* offsets,
                                            const int32_t* scan_of_pair, const int32_t* rows, const int32_t* cand,
                                            float* out_pts, int n_pairs, int N, int n_cand, void* stream) {
-  USIP_REQUIRE(scans && offsets && scan_of_pair && rows && cand && out_pts, "pair_gather_candidates: null pointer");
-  USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N, "pair_gather_candidates: bad sizes");
-  dim3 grid(cdiv(n_cand, 256), 2 * n_pairs);
-  pair_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of_pair, rows, cand, out_pts, N,
-                                                              n_cand);
-  return check_launch("pair_gather_kernel");
+  return pg_gather("pair_gather_candidates", scans, C, offsets, scan_of_pair, 1, rows, cand, out_pts, n_pairs, N,
+                   n_cand, stream);
+}
+
+extern "C" int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                                    int max_rows, int n_pairs, int N, int n_cand, uint64_t seed, uint64_t step,
+                                    int32_t* out_rows, int32_t* out_cand, int32_t* out_start, void* stream) {
+  return pg_subsample("cloud_subsample", scans, C, offsets, scan_of_cloud, 0, max_rows, n_pairs, N, n_cand, 0, 0.0,
+                      seed, step, out_rows, out_cand, out_start, nullptr, stream);
+}
+
+extern "C" int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets,
+                                            const int32_t* scan_of_cloud, const int32_t* rows, const int32_t* cand,
+                                            float* out_pts, int n_pairs, int N, int n_cand, void* stream) {
+  return pg_gather("cloud_gather_candidates", scans, C, offsets, scan_of_cloud, 0, rows, cand, out_pts, n_pairs, N,
+                   n_cand, stream);
+}
+
+extern "C" int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                                      const int32_t* rows, const float* nodes, const double* params,
+                                      const double* scale, const double* jit_pc, const double* jit_sn,
+                                      const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
+                                      int n_pairs, int N, int M, float* anc_pc, float* anc_sn, float* anc_node,
+                                      float* pos_pc, float* pos_sn, float* pos_node, void* stream) {
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes && params && scale, "desc_pair_augment: null input");
+  USIP_REQUIRE(anc_pc && anc_sn && anc_node && pos_pc && pos_sn && pos_node, "desc_pair_augment: null output");
+  USIP_REQUIRE(S >= 1 && S <= PG_MAX_S && 3 + S <= C, "desc_pair_augment: bad surface-normal length");
+  USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "desc_pair_augment: bad sizes");
+  dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
+  desc_pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
+      scans, C, offsets, scan_of_cloud, rows, nodes, params, scale, jit_pc, jit_sn, jit_node, seed, step, flags, S, N,
+      M, anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node);
+  return check_launch("desc_pair_augment_kernel");
 }
 
 extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,

@@ -287,10 +287,11 @@ def load_scan_npy(path, surface_normal_len):
     return np.ascontiguousarray(a, dtype=np.float32)
 
 
-def write_synthetic_kitti(root, counts, Ns, seed=0, C=8):
+def write_synthetic_kitti(root, counts, Ns, seed=0, C=8, poses=None):
     """A KITTI-shaped tree of seeded scans for tests and benchmarks: counts[seq] scans in sequence seq (0..10), each
     (Ns or Ns[seq][i], C) float32 [x, y, z, nx, ny, nz, curvature, reflectance] drawn from RandomState(seed + 1000*seq +
-    i), plus identity poses."""
+    i), plus poses: poses[seq][i] (4, 4) when given (a trajectory, for the descriptor's positives and negatives),
+    identity otherwise."""
     for seq, n in enumerate(counts):
         folder = os.path.join(root, "data_odometry_velodyne", "numpy", "%02d" % seq, KITTI_NP_FOLDER)
         os.makedirs(folder, exist_ok=True)
@@ -298,7 +299,8 @@ def write_synthetic_kitti(root, counts, Ns, seed=0, C=8):
         for i in range(n):
             ns = Ns if np.isscalar(Ns) else Ns[seq][i]
             np.save(os.path.join(folder, "%06d.npy" % i), synthetic_scan(seed + 1000 * seq + i, ns, C))
-            np.savez(os.path.join(root, "poses", "%02d" % seq, "%06d.npz" % i), pose=np.eye(4))
+            pose = np.eye(4) if poses is None else np.asarray(poses[seq][i])
+            np.savez(os.path.join(root, "poses", "%02d" % seq, "%06d.npz" % i), pose=pose)
 
 
 def synthetic_scan(seed, Ns, C=8):

@@ -202,6 +202,59 @@ def pair_augment(scans, offsets, scan_of_pair, rows, nodes, params, S, flags, se
     return out
 
 
+# ------------------------------------------------------------------------- descriptor training pairs (csrc/pairgen.cu)
+DESC_PARAM_STRIDE = 32
+
+
+def cloud_subsample(scans, offsets, scan_of_cloud, max_rows, N, n_cand, seed=0, step=0):
+    """Device-mode subsets of 2B clouds, each from its own scan.  scan_of_cloud (2B,) i32 ->
+    rows (2B, N) i32, cand (2B, n_cand) i32, start (2B,) i32.  Every scan must hold at least N rows."""
+    _req_scans(scans, offsets, scan_of_cloud)
+    B, dev = scan_of_cloud.shape[0] // 2, scans.device
+    rows = torch.empty((2 * B, int(N)), dtype=i32, device=dev)
+    cand = torch.empty((2 * B, int(n_cand)), dtype=i32, device=dev)
+    start = torch.empty((2 * B,), dtype=i32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_cloud_subsample(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), int(max_rows), B, int(N), int(n_cand),
+            int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), _p(rows), _p(cand), _p(start), _stream()),
+            "usip_cloud_subsample")
+    return rows, cand, start
+
+
+def cloud_gather_candidates(scans, offsets, scan_of_cloud, rows, cand):
+    """FPS input: (2B, n_cand, 3) f32 xyz of rows[c, cand[c, j]] of scan scan_of_cloud[c]."""
+    _req_scans(scans, offsets, scan_of_cloud); _req(rows, i32, "rows"); _req(cand, i32, "cand")
+    B, N, n_cand = scan_of_cloud.shape[0] // 2, rows.shape[1], cand.shape[1]
+    pts = torch.empty((2 * B, n_cand, 3), dtype=f32, device=scans.device)
+    with torch.cuda.device(scans.device):
+        check(_lib.load().usip_cloud_gather_candidates(_p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud),
+                                                       _p(rows), _p(cand), _p(pts), B, N, n_cand, _stream()),
+              "usip_cloud_gather_candidates")
+    return pts
+
+
+def desc_pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, scale, S, flags, seed=0, step=0,
+                      jit_pc=None, jit_sn=None, jit_node=None):
+    """Descriptor augmentation -> (anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node).  params (2B, 32) f64 per cloud,
+    scale (B,) f64 per pair, on the device (layout in include/usip_b200.h); jitter arrays f64 or None (drawn on the
+    device from (seed, step))."""
+    _req_scans(scans, offsets, scan_of_cloud); _req(rows, i32, "rows"); _req(nodes, f32, "nodes")
+    _req(params, torch.float64, "params"); _req(scale, torch.float64, "scale")
+    for name, j in (("jit_pc", jit_pc), ("jit_sn", jit_sn), ("jit_node", jit_node)):
+        if j is not None:
+            _req(j, torch.float64, name)
+    B, N, M, dev = scan_of_cloud.shape[0] // 2, rows.shape[1], nodes.shape[2], scans.device
+    e = lambda *s: torch.empty(s, dtype=f32, device=dev)
+    out = (e(B, 3, N), e(B, S, N), e(B, 3, M), e(B, 3, N), e(B, S, N), e(B, 3, M))
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_desc_pair_augment(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows), _p(nodes), _p(params), _p(scale),
+            _p(jit_pc), _p(jit_sn), _p(jit_node), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), int(flags),
+            int(S), B, N, M, *[_p(t) for t in out], _stream()), "usip_desc_pair_augment")
+    return out
+
+
 def nms(keypoints, sigmas, radius):
     """keypoints (B,3,M) f32, sigmas (B,M) f32 -> (idx (B,M) i32 kept indices in emission order, -1 padded; count (B,) i32)."""
     _req(keypoints, f32, "keypoints"); _req(sigmas, f32, "sigmas")
