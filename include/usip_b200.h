@@ -75,21 +75,26 @@ int usip_knn_group_f32(const float* xyz, const float* feat, const float* centers
 int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float* out_nodes, int B, int Ns, int k,
                  void* stream);
 
-/* Detector training pairs on the device (csrc/pairgen.cu)  data/kitti_detector_loader.py:101-259 (KittiLoader.__getitem__)
+/* Training pairs on the device (csrc/pairgen.cu): the detector's data/kitti_detector_loader.py:101-259
+ * (KittiLoader.__getitem__) and the descriptor's data/kitti_descriptor_loader.py:102-347
+ * (KittiDescriptorLoader.__getitem__).
  * Input: a ragged batch of raw scans, scans [T, C] f32 (x, y, z, then C-3 feature columns) with row offsets (n_scans+1)
- * i64; scan_of_pair (n_pairs) i32 names the scan of every pair.  Clouds are numbered c = 2*pair + side (0 = src, 1 = dst),
- * both sides subsample the same scan independently.  Every per-point random number is Philox4x32-10 keyed by
+ * i64.  Clouds are numbered c = 2*pair + side (0 = src / anchor, 1 = dst / positive); scan_of_cloud (2*n_pairs) i32 names
+ * the scan of every cloud.  The detector names a pair's scan twice (both sides subsample the same scan independently), the
+ * descriptor names the anchor's and the positive's.  Every per-point random number is Philox4x32-10 keyed by
  * (seed, step, cloud, point, purpose), so a batch is a pure function of (seed, step).
  *
- * usip_pair_subsample (get_instance_unaugmented_np, :118-145):
+ * usip_cloud_subsample (get_instance_unaugmented_np, detector :118-145, descriptor :117-128):
  *   out_rows (2*n_pairs, N) i32: row indices into each cloud's scan.  Optional radius mask (use_radius): fp32
  *     sqrt(x*x + z*z) compared in double against `radius`.  >= N points inside: a uniform subset of N without
  *     replacement, ascending row index.  Ns < N inside: every inside row t times (t the smallest >= 1 with Ns + t*Ns >= N),
  *     ascending, then a uniform subset of the N - t*Ns remainder, ascending.  A scan with no point inside gets rows 0.
+ *     (The descriptor's reference raises below N rows; its callers reject such scans.)
  *   out_cand (2*n_pairs, n_cand) i32: a uniform subset of n_cand of the N positions, ascending (the FPS candidates).
  *   out_start (2*n_pairs) i32: the FPS start index in [0, n_cand).  out_valid (2*n_pairs) i32: points inside (or NULL).
  *   max_rows >= the longest scan; max(max_rows, N) <= usip_pair_max_scan_rows().
- * usip_pair_gather_candidates: out_pts (2*n_pairs, n_cand, 3) f32 = xyz of rows[c, cand[c, j]] -- usip_fps_f32's input.
+ * usip_cloud_gather_candidates: out_pts (2*n_pairs, n_cand, 3) f32 = xyz of rows[c, cand[c, j]] of scan_of_cloud[c] --
+ *   usip_fps_f32's input.
  * usip_pair_augment (augment(), :149-216, train mode only, then transform_pc_pytorch for dst, augmentation.py:199-248):
  *   rows as above, nodes (2*n_pairs, 3, M) f32 = the FPS nodes (usip_fps_f32 out_nodes);
  *   params (n_pairs, 48) f64 per pair: [0:9] horizontal, [9:18] 3-d and [18:27] perturbation rotation matrices (row
@@ -99,52 +104,35 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *     it on the device (N(0, 0.04^2) clipped at 0.12 for pc / node, N(0, 0.01^2) clipped at 0.05 for sn);
  *   flags: USIP_PAIR_* below.  sn = columns 3:3+S of the scan, or the last column when S == 1.
  *   -> src/dst pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M), R (n_pairs, 3, 3), scale (n_pairs),
- *      shift (n_pairs, 3, 1), all f32 -- the nine tensors of ModelDetector.set_input. */
+ *      shift (n_pairs, 3, 1), all f32 -- the nine tensors of ModelDetector.set_input.
+ * usip_desc_pair_augment (augment(), :205-276, train mode only):
+ *   params (2*n_pairs, 32) f64 per cloud: [0:31] as above, with rotations and shift of the cloud's own and [27] the
+ *     pair's scale, the same value in both of its clouds;
+ *   jitter arrays and flags as in usip_pair_augment (the transform flags only); sn = columns 3:3+S for every S
+ *     (3 + S <= C).  Test mode (no USIP_PAIR_TRAIN): the rows and the nodes as they are.
+ *   -> anc/pos pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M) f32. */
 #define USIP_PAIR_TRAIN 1
 #define USIP_PAIR_ROT_HORIZONTAL 2
 #define USIP_PAIR_ROT_3D 4
 #define USIP_PAIR_ROT_PERTURBATION 8
 #define USIP_PAIR_TRANSLATION 16
 int usip_pair_max_scan_rows(void);
-int usip_pair_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair, int max_rows,
-                        int n_pairs, int N, int n_cand, int use_radius, double radius, uint64_t seed, uint64_t step,
-                        int32_t* out_rows, int32_t* out_cand, int32_t* out_start, int32_t* out_valid, void* stream);
-int usip_pair_gather_candidates(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,
-                                const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
-                                int n_cand, void* stream);
-int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,
+int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud, int max_rows,
+                         int n_pairs, int N, int n_cand, int use_radius, double radius, uint64_t seed, uint64_t step,
+                         int32_t* out_rows, int32_t* out_cand, int32_t* out_start, int32_t* out_valid, void* stream);
+int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                                 const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
+                                 int n_cand, void* stream);
+int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                       const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
                       const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
                       int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node, float* dst_pc,
                       float* dst_sn, float* dst_node, float* R, float* scale, float* shift, void* stream);
-
-/* Descriptor training pairs on the device (csrc/pairgen.cu)  data/kitti_descriptor_loader.py:102-347
- * (KittiDescriptorLoader.__getitem__).  Same scans / offsets / clouds as above, but the anchor (side 0) and the positive
- * (side 1) of a pair are different scans: scan_of_cloud (2*n_pairs) i32 names the scan of every cloud.  The Philox keys
- * are those of the detector calls for the same cloud number.
- *
- * usip_cloud_subsample (get_instance_unaugmented_np, :117-128): out_rows (2*n_pairs, N) i32, a uniform subset of N
- *   rows without replacement, ascending; out_cand (2*n_pairs, n_cand) i32 and out_start (2*n_pairs) i32 as in
- *   usip_pair_subsample.  No radius mask.  Every scan must hold at least N rows (the reference raises otherwise; the
- *   callers reject such scans); max_rows and the limit as in usip_pair_subsample.
- * usip_cloud_gather_candidates: out_pts (2*n_pairs, n_cand, 3) f32 = xyz of rows[c, cand[c, j]] of scan_of_cloud[c].
- * usip_desc_pair_augment (augment(), :205-276, train mode only):
- *   params (2*n_pairs, 32) f64 per cloud: [0:9] horizontal, [9:18] 3-d and [18:27] perturbation rotation matrices
- *     (row major, data @ R in float64), [28:31] the shift; [27] unused;  scale (n_pairs) f64 per pair;
- *   jitter arrays and flags as in usip_pair_augment (the transform flags only); sn = columns 3:3+S for every S
- *     (3 + S <= C).  Test mode (no USIP_PAIR_TRAIN): the rows and the nodes as they are.
- *   -> anc/pos pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M) f32. */
-int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud, int max_rows,
-                         int n_pairs, int N, int n_cand, uint64_t seed, uint64_t step, int32_t* out_rows,
-                         int32_t* out_cand, int32_t* out_start, void* stream);
-int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
-                                 const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
-                                 int n_cand, void* stream);
 int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
-                           const int32_t* rows, const float* nodes, const double* params, const double* scale,
-                           const double* jit_pc, const double* jit_sn, const double* jit_node, uint64_t seed,
-                           uint64_t step, int flags, int S, int n_pairs, int N, int M, float* anc_pc, float* anc_sn,
-                           float* anc_node, float* pos_pc, float* pos_sn, float* pos_node, void* stream);
+                           const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
+                           const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
+                           int n_pairs, int N, int M, float* anc_pc, float* anc_sn, float* anc_node, float* pos_pc,
+                           float* pos_sn, float* pos_node, void* stream);
 
 /* Radius non-maximum suppression of the detected keypoints    evaluation/save_keypoints.py:180-216 (nms)
  * keypoints (B,3,M) f32, sigmas (B,M) f32 -> out_idx (B,M) i32: original indices of the kept keypoints in the order the

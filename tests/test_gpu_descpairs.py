@@ -137,7 +137,7 @@ def test_device_subset_frequencies_chi_square():
         assert p > 1e-4, (n, chi2, p)
 
 
-def test_device_jitter_is_clipped_normal():
+def test_device_jitter_is_clipped_normal_with_the_scale_in_params():
     """With no rotation flag, scale 1 and no shift, output - input is the jitter (to fp32 rounding)."""
     N, M, S = 16384, 512, 4
     pc = np.random.RandomState(0).uniform(-1, 1, (2 * N, 8)).astype(np.float32)
@@ -147,8 +147,8 @@ def test_device_jitter_is_clipped_normal():
     rows = torch.arange(N, dtype=torch.int32, device=dev()).repeat(2, 1).contiguous()
     nodes = torch.from_numpy(np.stack([pc[:M, :3].T, pc[N:N + M, :3].T])).to(dev()).contiguous()
     params = torch.zeros((2, ops.DESC_PARAM_STRIDE), dtype=torch.float64, device=dev())
-    scale = torch.ones(1, dtype=torch.float64, device=dev())
-    out = ops.desc_pair_augment(scans, off, soc, rows, nodes, params, scale, S, ops.PAIR_TRAIN, seed=9, step=2)
+    params[:, 27] = 1
+    out = ops.desc_pair_augment(scans, off, soc, rows, nodes, params, S, ops.PAIR_TRAIN, seed=9, step=2)
     got = [t.cpu().numpy()[0].astype(np.float64) for t in out]
     j_pc = [got[0] - pc[:N, 0:3].T, got[3] - pc[N:, 0:3].T]
     j_sn = [got[1] - pc[:N, 3:3 + S].T, got[4] - pc[N:, 3:3 + S].T]

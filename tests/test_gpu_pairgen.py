@@ -134,13 +134,13 @@ def _clipped_std(sigma, clip):
     return sigma * math.sqrt((2 * Phi - 1) - 2 * c * phi + c * c * 2 * (1 - Phi))
 
 
-def test_device_jitter_is_clipped_normal():
+def test_device_jitter_is_clipped_normal_with_a_cloud_map():
     """With identity rotations, scale 1 and no shift, output - input is the jitter (to fp32 rounding)."""
     N, M, S = 16384, 512, 4
     pc = np.random.RandomState(0).uniform(-1, 1, (N, 8)).astype(np.float32)
     scans = torch.from_numpy(pc).to(dev())
     off = torch.tensor([0, N], dtype=torch.int64, device=dev())
-    sp = torch.zeros(1, dtype=torch.int32, device=dev())
+    sp = torch.zeros(2, dtype=torch.int32, device=dev())
     rows = torch.arange(N, dtype=torch.int32, device=dev()).repeat(2, 1).contiguous()
     nodes = torch.from_numpy(np.ascontiguousarray(pc[:M, :3].T)).to(dev()).repeat(2, 1, 1).contiguous()
     params = np.zeros((1, ops.PAIR_PARAM_STRIDE))
@@ -149,6 +149,8 @@ def test_device_jitter_is_clipped_normal():
     params[0, 43] = 1.0
     out = ops.pair_augment(scans, off, sp, rows, nodes, torch.from_numpy(params).to(dev()), S, ops.PAIR_TRAIN,
                            seed=9, step=2)
+    with pytest.raises(ValueError, match="both clouds"):               # a map with one entry per pair is refused
+        ops.pair_augment(scans, off, sp[:1], rows, nodes, torch.from_numpy(params).to(dev()), S, ops.PAIR_TRAIN)
     src_pc, src_sn, src_node = (t.cpu().numpy()[0].astype(np.float64) for t in out[:3])
     j_pc = src_pc - pc[:, 0:3].T
     j_sn = src_sn - pc[:, 3:3 + S].T

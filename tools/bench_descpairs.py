@@ -69,14 +69,14 @@ def bench_builder(a, dev, det):
     off_d = torch.from_numpy(off).to(dev)
     soc = torch.tensor(np.stack([anc, pos], 1).ravel(), dtype=torch.int32, device=dev)
     rows, cand, start = b.last["rows"], b.last["cand"], b.last["start"]
-    params, scale = b.last["params"], b.last["scale"]
+    params = b.last["params"]
     _, nodes = ops.fps(b.last["candidates"], start, M)
-    res["subsample_ms"] = event_ms(lambda: ops.cloud_subsample(scans, off_d, soc, a.scan_rows, N, b.n_cand, 1, 0),
+    res["subsample_ms"] = event_ms(lambda: ops.cloud_subsample(scans, off_d, soc, a.scan_rows, N, b.n_cand, seed=1),
                                    a.iters)
     res["gather_fps_ms"] = event_ms(lambda: ops.fps(ops.cloud_gather_candidates(scans, off_d, soc, rows, cand), start,
                                                     M), a.iters)
-    res["augment_ms"] = event_ms(lambda: ops.desc_pair_augment(scans, off_d, soc, rows, nodes, params, scale, S,
-                                                               b.flags, 1, 0), a.iters)
+    res["augment_ms"] = event_ms(lambda: ops.desc_pair_augment(scans, off_d, soc, rows, nodes, params, S, b.flags, 1,
+                                                               0), a.iters)
     # frozen detector on the built clouds
     out = b.build(scans, off, anc, pos, step=0)
     fn = lambda: det.run_model_siamese((out[0], out[3]), (out[1], out[4]), (out[2], out[5]))

@@ -56,14 +56,14 @@ def bench_builder(a, dev):
     res = {"batch_ms": event_ms(lambda: b.build(scans, off, items), a.iters)}
     # the three stages alone, on the inputs of one build
     off_d = torch.from_numpy(off).to(dev)
-    sp = torch.arange(B, dtype=torch.int32, device=dev)
+    sp = torch.arange(B, dtype=torch.int32, device=dev).repeat_interleave(2)      # both clouds of pair b: scan b
     rows, cand, start = b.last["rows"], b.last["cand"], b.last["start"]
     params = b.last["params"]
     _, nodes = ops.fps(b.last["candidates"], start, M)
-    res["subsample_ms"] = event_ms(lambda: ops.pair_subsample(scans, off_d, sp, a.scan_rows, N, b.n_cand, None, 1, 0),
+    res["subsample_ms"] = event_ms(lambda: ops.cloud_subsample(scans, off_d, sp, a.scan_rows, N, b.n_cand, None, 1, 0),
                                    a.iters)
-    res["gather_fps_ms"] = event_ms(lambda: ops.fps(ops.pair_gather_candidates(scans, off_d, sp, rows, cand), start, M),
-                                    a.iters)
+    res["gather_fps_ms"] = event_ms(lambda: ops.fps(ops.cloud_gather_candidates(scans, off_d, sp, rows, cand), start,
+                                                    M), a.iters)
     res["augment_ms"] = event_ms(lambda: ops.pair_augment(scans, off_d, sp, rows, nodes, params, S, b.flags, 1, 0),
                                  a.iters)
     # compulsory bytes of the augment kernel: row ids, the used scan columns and the nodes in; the nine outputs out

@@ -61,16 +61,13 @@ SIGNATURES = {
     "usip_layer_tile_rows": (c_int, []),
     "usip_fps_f32": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_pair_max_scan_rows": (c_int, []),
-    "usip_pair_subsample": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_int, c_int, c_int, c_int, c_int, ctypes.c_double,
-                                    ctypes.c_uint64, ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr]),
-    "usip_pair_gather_candidates": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                   ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
                           + [c_ptr] * 9 + [c_ptr]),
-    "usip_cloud_subsample": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_int, c_int, c_int, c_int, ctypes.c_uint64,
-                                     ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr]),
+    "usip_cloud_subsample": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_int, c_int, c_int, c_int, c_int, ctypes.c_double,
+                                     ctypes.c_uint64, ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr]),
     "usip_cloud_gather_candidates": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
-    "usip_desc_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
+    "usip_desc_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                        ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
                                + [c_ptr] * 6 + [c_ptr]),
     "usip_nms_f32":(c_int, [c_ptr, c_ptr, ctypes.c_float, c_ptr, c_ptr, c_int, c_int, c_ptr]),
@@ -155,7 +152,7 @@ def load():
 WEIGHT_GEN = [0]
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
-KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_pair_subsample": 2, "usip_cloud_subsample": 2}
+KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_cloud_subsample": 2}
 LAUNCHES = [0]
 
 

@@ -7,12 +7,10 @@
 // stream: the index lists and jitter arrays) or generated here with Philox4x32-10 keyed by (seed, step, cloud, point,
 // purpose), so that a batch is a pure function of (seed, step).
 //
-// Clouds are numbered c = 2*pair + side (side 0 = src / anchor, 1 = dst / positive).  The subset and gather kernels read
-// the scan of cloud c as scan_of[c >> pair_shift]: pair_shift = 1 for the detector (both sides of a pair subsample the
-// same scan), 0 for the descriptor (the anchor and the positive are different scans).  The Philox counters depend on c
-// only, so the mapping changes no random number.
-#include <stdio.h>
-
+// Clouds are numbered c = 2*pair + side (side 0 = src / anchor, 1 = dst / positive) and scan_of_cloud[c] names the scan
+// cloud c is drawn from: the detector names every pair's scan twice (both sides subsample the same scan), the
+// descriptor names the anchor's and the positive's.  The Philox counters depend on c only, so the mapping changes no
+// random number.
 #include "common.cuh"
 
 namespace usip {
@@ -136,17 +134,16 @@ __device__ __forceinline__ bool pg_inside(const float* p, double radius) {
 // level 1: the N/3 FPS candidates as ascending positions into the rows, and the FPS start index.
 __global__ void __launch_bounds__(PG_THREADS)
 pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
-                   const int32_t* __restrict__ scan_of, int pair_shift, int level, int use_radius, double radius, int N,
-                   int n_cand,
-                   uint64_t seed, uint64_t step, int32_t* __restrict__ out_rows, int32_t* __restrict__ out_cand,
-                   int32_t* __restrict__ out_start, int32_t* __restrict__ out_valid) {
+                   const int32_t* __restrict__ scan_of_cloud, int level, int use_radius, double radius, int N,
+                   int n_cand, uint64_t seed, uint64_t step, int32_t* __restrict__ out_rows,
+                   int32_t* __restrict__ out_cand, int32_t* __restrict__ out_start, int32_t* __restrict__ out_valid) {
   extern __shared__ __align__(16) unsigned char pg_smem[];
   __shared__ uint32_t hist[256];
   __shared__ uint32_t s_ctl[2];
   __shared__ uint64_t s_warp[32];
   uint32_t* key = reinterpret_cast<uint32_t*>(pg_smem);
   const int c = blockIdx.x, tid = threadIdx.x;
-  const int scan = scan_of[c >> pair_shift];
+  const int scan = scan_of_cloud[c];
   const int64_t row0 = offsets[scan];
   const int n = level == 0 ? (int)(offsets[scan + 1] - row0) : N;
   const float* base = scans + row0 * C;
@@ -214,12 +211,12 @@ pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __rest
 
 // candidate points for FPS: pts[c, j, :] = xyz of row rows[c, cand[c, j]]
 __global__ void pair_gather_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
-                                   const int32_t* __restrict__ scan_of, int pair_shift, const int32_t* __restrict__ rows,
+                                   const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
                                    const int32_t* __restrict__ cand, float* __restrict__ pts, int N, int n_cand) {
   const int c = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n_cand) return;
   const int r = rows[(int64_t)c * N + cand[(int64_t)c * n_cand + j]];
-  const float* p = scans + (offsets[scan_of[c >> pair_shift]] + r) * C;
+  const float* p = scans + (offsets[scan_of_cloud[c]] + r) * C;
   float* o = pts + ((int64_t)c * n_cand + j) * 3;
   o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
 }
@@ -355,7 +352,7 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
   }
 
   if (i < N) {
-    const int64_t row = offsets[scan_of_cloud[b]] + rows[(int64_t)c * N + i];
+    const int64_t row = offsets[scan_of_cloud[c]] + rows[(int64_t)c * N + i];
     const float* p = scans + row * C;
     float x = p[0], y = p[1], z = p[2];
     float sn[PG_MAX_S];
@@ -406,16 +403,16 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
 }
 
 // Descriptor pairs (KittiDescriptorLoader.augment, kitti_descriptor_loader.py:205-276): every cloud has its own scan,
-// rotations, jitter and shift; the scale is the pair's.  No dst transform.  sn = columns 3:3+S for every S.
+// rotations, jitter and shift; the scale is the pair's, in both clouds' [27].  No dst transform.  sn = columns 3:3+S
+// for every S.
 __global__ void __launch_bounds__(PG_AUG_THREADS)
 desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
                          const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
                          const float* __restrict__ nodes, const double* __restrict__ params,
-                         const double* __restrict__ scale, const double* __restrict__ jit_pc,
-                         const double* __restrict__ jit_sn, const double* __restrict__ jit_node, uint64_t seed,
-                         uint64_t step, int flags, int S, int N, int M, float* __restrict__ anc_pc,
-                         float* __restrict__ anc_sn, float* __restrict__ anc_node, float* __restrict__ pos_pc,
-                         float* __restrict__ pos_sn, float* __restrict__ pos_node) {
+                         const double* __restrict__ jit_pc, const double* __restrict__ jit_sn,
+                         const double* __restrict__ jit_node, uint64_t seed, uint64_t step, int flags, int S, int N,
+                         int M, float* __restrict__ anc_pc, float* __restrict__ anc_sn, float* __restrict__ anc_node,
+                         float* __restrict__ pos_pc, float* __restrict__ pos_sn, float* __restrict__ pos_node) {
   const int c = blockIdx.y, b = c >> 1, side = c & 1;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const double* P = params + (int64_t)c * PG_DESC_PARAM_STRIDE;
@@ -430,7 +427,7 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
     if (train) {
       double j[4];
       pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, j);
-      pg_augment_point(flags, P, scale[b], j, S, x, y, z, sn);
+      pg_augment_point(flags, P, P[27], j, S, x, y, z, sn);
       pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, sn);
     }
     float* opc = side ? pos_pc : anc_pc;
@@ -449,7 +446,7 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
     if (train) {
       double j[4];
       pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, j);
-      pg_augment_node(flags, P, scale[b], j, x, y, z);
+      pg_augment_node(flags, P, P[27], j, x, y, z);
     }
     float* ond = side ? pos_node : anc_node;
     ond[((int64_t)b * 3 + 0) * M + i] = x;
@@ -468,102 +465,65 @@ extern "C" int usip_pair_max_scan_rows(void) {
   return (227 * 1024 - 4096) / (int)sizeof(uint32_t);
 }
 
-// "<entry point>: <reason>" as the last error
-static int pg_fail(const char* what, const char* why) {
-  char msg[128];
-  snprintf(msg, sizeof(msg), "%s: %s", what, why);
-  set_last_error(msg);
-  return -1;
-}
-#define PG_REQUIRE(cond, why) do { if (!(cond)) return pg_fail(what, why); } while (0)
-
-// rows, then candidates + FPS start, of 2*n_pairs clouds (see the cloud -> scan mapping at the top)
-static int pg_subsample(const char* what, const float* scans, int C, const int64_t* offsets, const int32_t* scan_of,
-                        int pair_shift, int max_rows, int n_pairs, int N, int n_cand, int use_radius, double radius,
-                        uint64_t seed, uint64_t step, int32_t* out_rows, int32_t* out_cand, int32_t* out_start,
-                        int32_t* out_valid, void* stream) {
-  PG_REQUIRE(scans && offsets && scan_of && out_rows && out_cand && out_start, "null pointer");
-  PG_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N && max_rows > 0, "bad sizes");
-  const int smem = pg_subset_smem(max(max_rows, N));
-  PG_REQUIRE(max(max_rows, N) <= usip_pair_max_scan_rows(), "scan or N too large for shared memory");
-  cudaError_t e = cudaFuncSetAttribute(pair_subset_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (e != cudaSuccess) { pg_fail(what, "smem attribute"); return (int)e; }
+// rows, then candidates + FPS start, of 2*n_pairs clouds
+extern "C" int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                                    int max_rows, int n_pairs, int N, int n_cand, int use_radius, double radius,
+                                    uint64_t seed, uint64_t step, int32_t* out_rows, int32_t* out_cand,
+                                    int32_t* out_start, int32_t* out_valid, void* stream) {
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && out_rows && out_cand && out_start, "cloud_subsample: null pointer");
+  USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N && max_rows > 0,
+               "cloud_subsample: bad sizes");
+  USIP_REQUIRE(max(max_rows, N) <= usip_pair_max_scan_rows(),
+               "cloud_subsample: scan or N too large for shared memory");
+  cudaError_t e = cudaFuncSetAttribute(pair_subset_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       pg_subset_smem(max(max_rows, N)));
+  if (e != cudaSuccess) { set_last_error("cloud_subsample: smem attribute"); return (int)e; }
   cudaStream_t s = (cudaStream_t)stream;
   pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(max_rows), s>>>(
-      scans, C, offsets, scan_of, pair_shift, 0, use_radius, radius, N, n_cand, seed, step, out_rows, out_cand,
-      out_start, out_valid);
+      scans, C, offsets, scan_of_cloud, 0, use_radius, radius, N, n_cand, seed, step, out_rows, out_cand, out_start,
+      out_valid);
   int rc = check_launch("pair_subset_kernel(rows)");
   if (rc) return rc;
   pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(N), s>>>(
-      scans, C, offsets, scan_of, pair_shift, 1, 0, 0.0, N, n_cand, seed, step, out_rows, out_cand, out_start,
-      out_valid);
+      scans, C, offsets, scan_of_cloud, 1, 0, 0.0, N, n_cand, seed, step, out_rows, out_cand, out_start, out_valid);
   return check_launch("pair_subset_kernel(candidates)");
-}
-
-static int pg_gather(const char* what, const float* scans, int C, const int64_t* offsets, const int32_t* scan_of,
-                     int pair_shift, const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
-                     int n_cand, void* stream) {
-  PG_REQUIRE(scans && offsets && scan_of && rows && cand && out_pts, "null pointer");
-  PG_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N, "bad sizes");
-  dim3 grid(cdiv(n_cand, 256), 2 * n_pairs);
-  pair_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of, pair_shift, rows, cand,
-                                                              out_pts, N, n_cand);
-  return check_launch("pair_gather_kernel");
-}
-
-extern "C" int usip_pair_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,
-                                   int max_rows, int n_pairs, int N, int n_cand, int use_radius, double radius,
-                                   uint64_t seed, uint64_t step, int32_t* out_rows, int32_t* out_cand,
-                                   int32_t* out_start, int32_t* out_valid, void* stream) {
-  return pg_subsample("pair_subsample", scans, C, offsets, scan_of_pair, 1, max_rows, n_pairs, N, n_cand, use_radius,
-                      radius, seed, step, out_rows, out_cand, out_start, out_valid, stream);
-}
-
-extern "C" int usip_pair_gather_candidates(const float* scans, int C, const int64_t* offsets,
-                                           const int32_t* scan_of_pair, const int32_t* rows, const int32_t* cand,
-                                           float* out_pts, int n_pairs, int N, int n_cand, void* stream) {
-  return pg_gather("pair_gather_candidates", scans, C, offsets, scan_of_pair, 1, rows, cand, out_pts, n_pairs, N,
-                   n_cand, stream);
-}
-
-extern "C" int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
-                                    int max_rows, int n_pairs, int N, int n_cand, uint64_t seed, uint64_t step,
-                                    int32_t* out_rows, int32_t* out_cand, int32_t* out_start, void* stream) {
-  return pg_subsample("cloud_subsample", scans, C, offsets, scan_of_cloud, 0, max_rows, n_pairs, N, n_cand, 0, 0.0,
-                      seed, step, out_rows, out_cand, out_start, nullptr, stream);
 }
 
 extern "C" int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets,
                                             const int32_t* scan_of_cloud, const int32_t* rows, const int32_t* cand,
                                             float* out_pts, int n_pairs, int N, int n_cand, void* stream) {
-  return pg_gather("cloud_gather_candidates", scans, C, offsets, scan_of_cloud, 0, rows, cand, out_pts, n_pairs, N,
-                   n_cand, stream);
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && cand && out_pts, "cloud_gather_candidates: null pointer");
+  USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N, "cloud_gather_candidates: bad sizes");
+  dim3 grid(cdiv(n_cand, 256), 2 * n_pairs);
+  pair_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of_cloud, rows, cand, out_pts, N,
+                                                              n_cand);
+  return check_launch("pair_gather_kernel");
 }
 
 extern "C" int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                                       const int32_t* rows, const float* nodes, const double* params,
-                                      const double* scale, const double* jit_pc, const double* jit_sn,
-                                      const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
-                                      int n_pairs, int N, int M, float* anc_pc, float* anc_sn, float* anc_node,
-                                      float* pos_pc, float* pos_sn, float* pos_node, void* stream) {
-  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes && params && scale, "desc_pair_augment: null input");
+                                      const double* jit_pc, const double* jit_sn, const double* jit_node,
+                                      uint64_t seed, uint64_t step, int flags, int S, int n_pairs, int N, int M,
+                                      float* anc_pc, float* anc_sn, float* anc_node, float* pos_pc, float* pos_sn,
+                                      float* pos_node, void* stream) {
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes && params, "desc_pair_augment: null input");
   USIP_REQUIRE(anc_pc && anc_sn && anc_node && pos_pc && pos_sn && pos_node, "desc_pair_augment: null output");
   USIP_REQUIRE(S >= 1 && S <= PG_MAX_S && 3 + S <= C, "desc_pair_augment: bad surface-normal length");
   USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "desc_pair_augment: bad sizes");
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
   desc_pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
-      scans, C, offsets, scan_of_cloud, rows, nodes, params, scale, jit_pc, jit_sn, jit_node, seed, step, flags, S, N,
-      M, anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node);
+      scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, N, M,
+      anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node);
   return check_launch("desc_pair_augment_kernel");
 }
 
-extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_pair,
+extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                                  const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
                                  const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags,
                                  int S, int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node,
                                  float* dst_pc, float* dst_sn, float* dst_node, float* R, float* scale, float* shift,
                                  void* stream) {
-  USIP_REQUIRE(scans && offsets && scan_of_pair && rows && nodes && params, "pair_augment: null input");
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes && params, "pair_augment: null input");
   USIP_REQUIRE(src_pc && src_sn && src_node && dst_pc && dst_sn && dst_node && R && scale && shift,
                "pair_augment: null output");
   USIP_REQUIRE(S >= 1 && S <= PG_MAX_S && (S == 1 || 3 + S <= C) && C >= 4, "pair_augment: bad surface-normal length");
@@ -571,7 +531,7 @@ extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offse
   const int sn_col = S == 1 ? C - 1 : 3;           // kitti_detector_loader.py:135-139
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
   pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
-      scans, C, offsets, scan_of_pair, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, sn_col, N,
+      scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, sn_col, N,
       M, src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, R, scale, shift);
   return check_launch("pair_augment_kernel");
 }

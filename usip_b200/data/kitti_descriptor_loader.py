@@ -5,7 +5,7 @@ The descriptor is trained on keypoints of the frozen detector.  Each item is an 
 within `positive_radius_threshold` of it, both subsampled, given FPS nodes and augmented; the frozen detector turns
 every cloud into keypoints and sigmas, and the negatives are other anchors of the batch more than
 `negative_radius_threshold` away.  `DescriptorPairBuilder` builds the clouds on the device (csrc/pairgen.cu: the
-subset and candidate kernels of the detector builder with one scan per cloud, and `usip_desc_pair_augment`);
+per-cloud subset and candidate kernels the detector builder uses, and `usip_desc_pair_augment`);
 `KittiDescriptorPairSource` adds the positive search, the frozen detector pass and negative mining, and hands the nine
 `ModelDescriptor.set_input` tensors over without a host synchronise.
 """
@@ -18,8 +18,7 @@ import torch
 
 from usip_b200 import ops
 
-from .kitti_detector_loader import (FPS_MAX_CANDIDATES, _step_rng, angles2rotation_matrix, draw_subsample,
-                                    kitti_scan_path, load_scan_npy, make_dataset_kitti)
+from .kitti_detector_loader import _KittiSource, _PairBuilder, angles2rotation_matrix, make_dataset_kitti
 
 DESC_DIVISOR = 4                                 # kitti_descriptor_loader.py:127: FPS over N/4 candidates
 
@@ -110,7 +109,7 @@ def draw_desc_pair_scalars(rng, train, N, M, S, per_point):
 
 
 # ----------------------------------------------------------------------------------------------- the builder
-class DescriptorPairBuilder:
+class DescriptorPairBuilder(_PairBuilder):
     """Builds the six cloud tensors (anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node) of a batch of KITTI
     descriptor pairs on the device.
 
@@ -118,120 +117,42 @@ class DescriptorPairBuilder:
     scans are uploaded), offsets (n_scans+1,) int64 row offsets (host), anc_items / pos_items the scan index of every
     anchor and positive.  Every scan needs at least input_pc_num rows: the reference draws them without replacement.
 
-    rng="device": per-point randomness is Philox keyed by (seed, step, cloud, point, purpose), per-pair scalars come
-    from a numpy RandomState seeded by (seed, step): a batch is a pure function of (seed, step), with O(B) host work.
-    Selected rows ascend (see usip_cloud_subsample in include/usip_b200.h).
-    rng="numpy": parity mode.  Consumes the global np.random exactly as KittiDescriptorLoader.__getitem__ does, item by
-    item (anchor rows, candidates, FPS start; positive the same; then the augmentation), and uploads the index lists and
-    jitter arrays.  The positive search draws from Python's `random` only, so choosing pos_items beforehand with
-    `nearby_index` changes no numpy draw.
-
-    The outputs are fresh tensors allocated on the current stream.  `last` keeps the index lists of the last build.
+    See `_PairBuilder` for the two rng modes; rng="numpy" replays KittiDescriptorLoader.__getitem__.  The positive
+    search draws from Python's `random` only, so choosing pos_items beforehand with `nearby_index` changes no numpy
+    draw.  `last` keeps the index lists of the last build, and the pairs' scales.
     """
 
     def __init__(self, opt, mode="train", device=None, seed=0, rng="device"):
-        if mode not in ("train", "test"):
-            raise ValueError("mode must be 'train' or 'test'")
-        if rng not in ("device", "numpy"):
-            raise ValueError("rng must be 'device' or 'numpy'")
-        self.opt, self.mode, self.rng, self.seed = opt, mode, rng, int(seed)
-        self.device = torch.device(device if device is not None else "cuda")
-        self.N, self.M, self.S = int(opt.input_pc_num), int(opt.node_num), int(opt.surface_normal_len)
-        self.n_cand = int(self.N / DESC_DIVISOR)
-        if self.n_cand > FPS_MAX_CANDIDATES:
-            raise ValueError("input_pc_num / %d = %d FPS candidates; usip_fps_f32 takes at most %d"
-                             % (DESC_DIVISOR, self.n_cand, FPS_MAX_CANDIDATES))
-        if self.n_cand < 1 or self.M > self.n_cand:
-            raise ValueError("node_num %d needs at least as many FPS candidates (%d)" % (self.M, self.n_cand))
+        super().__init__(opt, mode, device, seed, rng, DESC_DIVISOR)
         if not 1 <= self.S <= 8:
             raise ValueError("surface_normal_len %d: the augment kernel takes 1..8" % self.S)
-        self.flags = ((ops.PAIR_TRAIN if mode == "train" else 0)
-                      | (ops.PAIR_ROT_HORIZONTAL if getattr(opt, "rot_horizontal", False) else 0)
-                      | (ops.PAIR_ROT_3D if getattr(opt, "rot_3d", False) else 0)
-                      | (ops.PAIR_ROT_PERTURBATION if getattr(opt, "rot_perturbation", False) else 0)
-                      | (ops.PAIR_TRANSLATION if getattr(opt, "translation_perturbation", False) else 0))
-        self.step = 0
-        self.last = None
 
-    def _check(self, scans, offsets, anc_items, pos_items):
-        offsets = np.asarray(offsets, dtype=np.int64)
-        if offsets.ndim != 1 or offsets.shape[0] < 2:
-            raise ValueError("no scans")
+    def _clouds(self, anc_items, pos_items):
         anc = np.asarray(anc_items, dtype=np.int64).ravel()
         pos = np.asarray(pos_items, dtype=np.int64).ravel()
         if anc.size == 0:
             raise ValueError("no items")
         if anc.shape != pos.shape:
             raise ValueError("%d anchors but %d positives" % (anc.size, pos.size))
-        clouds = np.stack([anc, pos], 1).ravel()              # cloud 2b = anchor b, 2b+1 = its positive
-        if clouds.min() < 0 or clouds.max() >= offsets.shape[0] - 1:
-            raise IndexError("item out of range")
-        lengths = offsets[clouds + 1] - offsets[clouds]
+        return np.stack([anc, pos], 1).ravel()                # cloud 2b = anchor b, 2b+1 = its positive
+
+    def _check_rows(self, clouds, lengths):
         k = int(np.argmin(lengths))
-        if lengths[k] <= 0:
-            raise ValueError("scan %d has no points" % int(clouds[k]))
         if lengths[k] < self.N:
             raise ValueError("scan %d has %d rows; input_pc_num = %d rows are drawn without replacement"
                              % (int(clouds[k]), int(lengths[k]), self.N))
-        C = scans.shape[1]
-        if scans.dim() != 2 or C < 3 + self.S:
-            raise ValueError("scans have %d columns, surface_normal_len %d needs %d" % (C, self.S, 3 + self.S))
-        max_rows = int(lengths.max())
-        if max_rows > ops.pair_max_scan_rows():
-            raise ValueError("a scan of %d rows exceeds the %d the subsample kernel holds"
-                             % (max_rows, ops.pair_max_scan_rows()))
-        return offsets, clouds, lengths, max_rows
+
+    def _draw(self, rng, per_point):
+        p, _, jit = draw_desc_pair_scalars(rng, self.mode == "train", self.N, self.M, self.S, per_point)
+        return p, jit
+
+    def _augment(self, scans, offsets, scan_of_cloud, rows, nodes, params, step, jit):
+        return ops.desc_pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, self.S, self.flags, self.seed,
+                                     step, *jit)
 
     def build(self, scans, offsets, anc_items, pos_items, step=None):
-        offsets, clouds, lengths, max_rows = self._check(scans, offsets, anc_items, pos_items)
-        if step is None:
-            step = self.step
-        self.step = int(step) + 1
-        B, N, M, S, dev = len(clouds) // 2, self.N, self.M, self.S, self.device
-        train = self.mode == "train"
-
-        host_scans = None
-        if self.rng == "numpy":
-            host_scans = [scans[offsets[i]:offsets[i + 1]].cpu().numpy() for i in clouds]
-        if scans.device != dev:                        # upload only the scans this batch uses, each once
-            uniq, inv = np.unique(clouds, return_inverse=True)
-            parts = [scans[offsets[i]:offsets[i + 1]] for i in uniq]
-            scans = torch.cat(parts).pin_memory().to(dev, non_blocking=True)
-            offsets = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
-            clouds = inv.astype(np.int64).ravel()
-        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
-        offsets_d = up(offsets)
-        scan_of_cloud = up(clouds.astype(np.int32))
-
-        jit = (None, None, None)
-        with torch.cuda.device(dev):
-            if self.rng == "device":
-                rows, cand, start = ops.cloud_subsample(scans, offsets_d, scan_of_cloud, max_rows, N, self.n_cand,
-                                                        self.seed, step)
-                hrng = _step_rng(self.seed, step)
-                drawn = [draw_desc_pair_scalars(hrng, train, N, M, S, False) for _ in range(B)]
-            else:
-                rows_h = np.empty((2 * B, N), np.int32)
-                cand_h = np.empty((2 * B, self.n_cand), np.int32)
-                start_h = np.empty((2 * B,), np.int32)
-                drawn = []
-                for b in range(B):                     # KittiDescriptorLoader.__getitem__, item by item
-                    for side in range(2):              # anchor, then positive (:321-323)
-                        c = 2 * b + side
-                        rows_h[c], cand_h[c], start_h[c] = draw_subsample(np.random, len(host_scans[c]), N,
-                                                                          DESC_DIVISOR)
-                    drawn.append(draw_desc_pair_scalars(np.random, train, N, M, S, True))
-                rows, cand, start = up(rows_h), up(cand_h), up(start_h)
-                if train:
-                    jit = tuple(up(np.stack([d[2][k] for d in drawn]).reshape((2 * B,) + drawn[0][2][k].shape[1:]))
-                                for k in range(3))
-            params = up(np.concatenate([d[0] for d in drawn]))
-            scale = up(np.array([d[1] for d in drawn], dtype=np.float64))
-            pts = ops.cloud_gather_candidates(scans, offsets_d, scan_of_cloud, rows, cand)
-            _, nodes = ops.fps(pts, start, M, want_nodes=True)
-            out = ops.desc_pair_augment(scans, offsets_d, scan_of_cloud, rows, nodes, params, scale, S, self.flags,
-                                        self.seed, step, *jit)
-        self.last = {"rows": rows, "cand": cand, "start": start, "candidates": pts, "params": params, "scale": scale}
+        out = self._build(scans, offsets, step, anc_items, pos_items)
+        self.last["scale"] = self.last["params"][0::2, 27]    # a pair's scale is in both of its clouds' blocks
         return out
 
 
@@ -250,15 +171,13 @@ def load_kitti_poses(root, mode):
     return seq, (np.stack(poses) if poses else np.zeros((0, 4, 4)))
 
 
-class KittiDescriptorPairSource:
+class KittiDescriptorPairSource(_KittiSource):
     """Shuffled batches of KITTI descriptor training inputs, built on the device, for `ModelDescriptor`.
 
-    Scans are indexed like make_dataset_kitti and loaded once into pinned host memory (or onto the device with
-    resident="device"), the poses once into a host array.  For every batch, on a stream of its own: shuffle the
-    anchors, pick each positive with `nearby_index` (host, Python's random), build the clouds (`DescriptorPairBuilder`),
-    run the frozen `detector.run_model_siamese` on the built nodes for keypoints and sigmas, and mine the negatives
-    (host, float32 poses).  Batch i+1 is built while the caller runs step i; `feed()` hands each batch over with
-    `model.prefetch_input(..., after=event)` + `set_input()`, so the host never synchronises.
+    Scans and hand-over as in `_KittiSource`; the poses are loaded once into a host array.  For every batch, on the
+    build stream: pick each anchor's positive with `nearby_index` (host, Python's random), build the clouds
+    (`DescriptorPairBuilder`), run the frozen `detector.run_model_siamese` on the built nodes for keypoints and sigmas,
+    and mine the negatives (host, float32 poses).
 
         src = KittiDescriptorPairSource(root, "train", opt, detector)
         for epoch in range(E):
@@ -268,69 +187,24 @@ class KittiDescriptorPairSource:
 
     def __init__(self, root, mode, opt, detector, device=None, seed=0, resident="host", rng="device",
                  batch_size=None, drop_last=True):
-        self.opt, self.mode, self.detector = opt, mode, detector
-        self.device = torch.device(device if device is not None else "cuda")
-        self.batch_size = int(batch_size or opt.batch_size)
-        self.drop_last = drop_last
+        super().__init__(root, mode, opt, DescriptorPairBuilder, device, seed, resident, rng, batch_size, drop_last)
+        self.detector = detector
         self.pos_threshold = float(getattr(opt, "positive_radius_threshold", 5.0))
         self.neg_threshold = float(getattr(opt, "negative_radius_threshold", 50.0))
-        _, _, self.nums, self.accs = make_dataset_kitti(root, mode)
-        n = self.accs[-1] if self.accs else 0
-        if n == 0:
-            raise ValueError("no scans under %s" % root)
-        arrs = [load_scan_npy(kitti_scan_path(root, mode, i), opt.surface_normal_len) for i in range(n)]
-        if len({a.shape[1] for a in arrs}) != 1:
-            raise ValueError("scans differ in column count")
         self.seq, self.poses = load_kitti_poses(root, mode)
-        self.offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrs])]).astype(np.int64)
-        scans = torch.from_numpy(np.concatenate(arrs))
-        self.scans = scans.to(self.device) if resident == "device" else scans.pin_memory()
-        self.builder = DescriptorPairBuilder(opt, mode, self.device, seed, rng)
-        self.order_rng = np.random.RandomState(seed)
         self.pos_rng = random.Random(seed)
         self.neg_rng = np.random.RandomState(seed + 1)
-        self.stream = torch.cuda.Stream(device=self.device)
-        self.step = 0
-        self.last = None                        # what the batch last yielded was built from, for inspection
-
-    def __len__(self):
-        n = len(self.offsets) - 1
-        return n // self.batch_size if self.drop_last else -(-n // self.batch_size)
 
     def _build(self, anchors):
         pos = [nearby_index(int(a), self.poses, self.accs, self.nums, self.pos_threshold, self.pos_rng)
                for a in anchors]
         neg = mine_negative_sample(self.seq[anchors], self.poses[anchors].astype(np.float32), self.neg_threshold,
                                    self.neg_rng)
-        with torch.cuda.stream(self.stream):
-            anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node = self.builder.build(self.scans, self.offsets, anchors,
-                                                                                    pos, step=self.step)
-            (anc_kp, pos_kp), (anc_sig, pos_sig) = self.detector.run_model_siamese((anc_pc, pos_pc), (anc_sn, pos_sn),
-                                                                                   (anc_node, pos_node))
-            neg_d = neg.pin_memory().to(self.device, non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(self.stream)
-        self.step += 1
+        anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node = self.builder.build(self.scans, self.offsets, anchors, pos,
+                                                                                step=self.step)
+        (anc_kp, pos_kp), (anc_sig, pos_sig) = self.detector.run_model_siamese((anc_pc, pos_pc), (anc_sn, pos_sn),
+                                                                               (anc_node, pos_node))
+        neg_d = neg.pin_memory().to(self.device, non_blocking=True)
         info = {"anchors": np.asarray(anchors), "positives": np.asarray(pos), "neg_idx": neg,
                 "clouds": (anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node)}
-        return (anc_pc, anc_sn, anc_kp, anc_sig, pos_pc, pos_sn, pos_kp, pos_sig, neg_d), ev, info
-
-    def batches(self):
-        """One shuffled epoch of (nine set_input tensors, ready event); batch i+1 is enqueued before batch i is
-        yielded."""
-        perm = self.order_rng.permutation(len(self.offsets) - 1)
-        chunks = [perm[i:i + self.batch_size] for i in range(0, len(perm), self.batch_size)]
-        if self.drop_last and chunks and len(chunks[-1]) < self.batch_size:
-            chunks.pop()
-        nxt = self._build(chunks[0]) if chunks else None
-        for k in range(len(chunks)):
-            out, ev, self.last = nxt
-            nxt = self._build(chunks[k + 1]) if k + 1 < len(chunks) else None
-            yield out, ev
-
-    def feed(self, model):
-        """One epoch; before each yield the batch is the model's input (prefetch_input + set_input)."""
-        for out, ev in self.batches():
-            model.prefetch_input(*out, after=ev)
-            model.set_input(*out)
-            yield out
+        return (anc_pc, anc_sn, anc_kp, anc_sig, pos_pc, pos_sn, pos_kp, pos_sig, neg_d), info

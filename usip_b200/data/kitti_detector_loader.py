@@ -4,8 +4,8 @@
 whole training batch of `KittiLoader.__getitem__` (:218-259) on the device -- random subsampling, FPS nodes,
 augmentation and the dst transform -- and `KittiPairSource` feeds such batches to `ModelDetector` from a KITTI tree.
 The reference runs all of this per pair in DataLoader workers: serial numpy, more host time per pair than a whole
-training step of this repository.  Only the KITTI detector loader is covered; the Oxford / ModelNet / SceneNN / Match3D
-loaders differ in the candidate divisor (a parameter here) and in using two scans.
+training step of this repository.  Only the KITTI loaders are covered (the descriptor's builds on the bases here); the
+Oxford / ModelNet / SceneNN / Match3D loaders differ in the candidate divisor (a parameter here) and in using two scans.
 """
 import os
 
@@ -125,25 +125,27 @@ def _step_rng(seed, step):
     return np.random.RandomState(np.array(w, dtype=np.uint32))
 
 
-# ----------------------------------------------------------------------------------------------- the builder
-class DetectorPairBuilder:
-    """Builds the nine `ModelDetector.set_input` tensors of a batch of KITTI pairs on the device.
-
-    `build(scans, offsets, items, step=None)`: scans [T, C] f32 (device, or host -- then the items' scans are uploaded),
-    offsets (n_scans+1,) int64 row offsets (host), items the scan index of every pair.  Both clouds of a pair are
-    independent subsamples of the same scan (kitti_detector_loader.py:219-220).
+# ----------------------------------------------------------------------------------------------- the builders
+class _PairBuilder:
+    """What the detector's and the descriptor's pair builders share.  A batch of B pairs is 2B clouds, cloud 2b + side
+    (side 0 = src / anchor, 1 = dst / positive) a subsample of one scan: subsets, FPS candidates and nodes are built per
+    cloud, whichever scans a pair's two clouds come from.  A subclass names the scan of every cloud (`_clouds`), draws
+    one pair's scalars (`_draw`) and runs its augment kernel (`_augment`).
 
     rng="device": per-point randomness (subsets, jitter, FPS start) is Philox keyed by (seed, step, cloud, point,
     purpose); per-pair scalars come from a numpy RandomState seeded by (seed, step).  Host work is O(B) and a given
     (seed, step) always gives the same batch, bit for bit.  Selected rows ascend within each part (see
-    usip_pair_subsample in include/usip_b200.h); the reference's order is numpy's permutation order.
-    rng="numpy": parity mode.  Consumes the global np.random exactly as KittiLoader.__getitem__ does, item by item,
-    and uploads the index lists and jitter arrays: slow by design, it reproduces the reference's batch.
+    usip_cloud_subsample in include/usip_b200.h); the reference's order is numpy's permutation order.
+    rng="numpy": parity mode.  Consumes the global np.random exactly as the reference's __getitem__ does, item by item
+    (side 0's rows, candidates and FPS start, side 1's, then the pair's augmentation), and uploads the index lists and
+    jitter arrays: slow by design, it reproduces the reference's batch.
 
     The outputs are fresh tensors allocated on the current stream; nothing is overwritten by a later build.
     """
 
-    def __init__(self, opt, mode="train", device=None, seed=0, rng="device", divisor=3):
+    radius = None                                # only rows within this xz distance of the sensor are drawable
+
+    def __init__(self, opt, mode, device, seed, rng, divisor):
         if mode not in ("train", "test"):
             raise ValueError("mode must be 'train' or 'test'")
         if rng not in ("device", "numpy"):
@@ -158,8 +160,6 @@ class DetectorPairBuilder:
                              % (divisor, self.n_cand, FPS_MAX_CANDIDATES))
         if self.n_cand < 1 or self.M > self.n_cand:
             raise ValueError("node_num %d needs at least as many FPS candidates (%d)" % (self.M, self.n_cand))
-        r = getattr(opt, "radius_threshold", 100.0)
-        self.radius = float(r) if r < 90 else None
         self.flags = ((ops.PAIR_TRAIN if mode == "train" else 0)
                       | (ops.PAIR_ROT_HORIZONTAL if getattr(opt, "rot_horizontal", False) else 0)
                       | (ops.PAIR_ROT_3D if getattr(opt, "rot_3d", False) else 0)
@@ -168,86 +168,119 @@ class DetectorPairBuilder:
         self.step = 0
         self.last = None                      # index lists of the last build (rows, cand, start), for inspection
 
-    def _check(self, offsets, items):
+    def _clouds(self, *items):
+        """(2B,) int64: the scan of every cloud."""
+        raise NotImplementedError
+
+    def _check_rows(self, clouds, lengths):
+        """Reject scans too short for the subclass's loader (every scan here has at least one row)."""
+
+    def _draw(self, rng, per_point):
+        """One pair's scalars -> (params block, jitter (pc (2,N,3), sn (2,N,S), node (2,M,3)) or None)."""
+        raise NotImplementedError
+
+    def _augment(self, scans, offsets, scan_of_cloud, rows, nodes, params, step, jit):
+        raise NotImplementedError
+
+    def _build(self, scans, offsets, step, *items):
         offsets = np.asarray(offsets, dtype=np.int64)
         if offsets.ndim != 1 or offsets.shape[0] < 2:
             raise ValueError("no scans")
-        items = np.asarray(items, dtype=np.int64).ravel()
-        if items.size == 0:
-            raise ValueError("no items")
-        if items.min() < 0 or items.max() >= offsets.shape[0] - 1:
+        clouds = self._clouds(*items)
+        if clouds.min() < 0 or clouds.max() >= offsets.shape[0] - 1:
             raise IndexError("item out of range")
-        lengths = offsets[items + 1] - offsets[items]
-        if lengths.min() <= 0:
-            raise ValueError("scan %d has no points" % int(items[np.argmin(lengths)]))
-        return offsets, items, lengths
-
-    def build(self, scans, offsets, items, step=None):
-        offsets, items, lengths = self._check(offsets, items)
-        if step is None:
-            step = self.step
-        self.step = int(step) + 1
-        B, N, M, S, dev = len(items), self.N, self.M, self.S, self.device
+        lengths = offsets[clouds + 1] - offsets[clouds]
+        k = int(np.argmin(lengths))
+        if lengths[k] <= 0:
+            raise ValueError("scan %d has no points" % int(clouds[k]))
+        self._check_rows(clouds, lengths)
+        B, N, M, S, dev = len(clouds) // 2, self.N, self.M, self.S, self.device
+        C = scans.shape[1]
+        if scans.dim() != 2 or C < 3 + max(S, 1):
+            raise ValueError("scans have %d columns, surface_normal_len %d needs %d" % (C, S, 3 + S))
         max_rows = int(max(lengths.max(), N))
         if max_rows > ops.pair_max_scan_rows():
             raise ValueError("a scan of %d rows exceeds the %d the subsample kernel holds"
                              % (max_rows, ops.pair_max_scan_rows()))
-        C = scans.shape[1]
-        if C < 3 + max(S, 1) or (S == 1 and C < 4):
-            raise ValueError("scans have %d columns, surface_normal_len %d needs %d" % (C, S, 3 + S))
+        if step is None:
+            step = self.step
+        self.step = int(step) + 1
 
-        host_scans = None
-        if scans.device != dev:                        # upload only the scans this batch uses
-            if self.rng == "numpy":
-                host_scans = [scans[offsets[i]:offsets[i + 1]].numpy() for i in items]
-            parts = [scans[offsets[i]:offsets[i + 1]] for i in items]
+        used = np.unique(clouds)
+        drawable = None                                # parity mode with a radius: the rows inside it, per cloud
+        if self.rng == "numpy" and self.radius is not None:
+            inside = {i: np.nonzero(radius_mask(scans[offsets[i]:offsets[i + 1]].cpu().numpy(), self.radius))[0]
+                      for i in used}
+            drawable = [inside[i] for i in clouds]
+        if scans.device != dev:                        # upload only the scans this batch uses, each once
+            parts = [scans[offsets[i]:offsets[i + 1]] for i in used]
             scans = torch.cat(parts).pin_memory().to(dev, non_blocking=True)
-            offsets = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
-            items = np.arange(B, dtype=np.int64)
-        elif self.rng == "numpy":
-            host_scans = [scans[offsets[i]:offsets[i + 1]].cpu().numpy() for i in items]
-        offsets_d = torch.from_numpy(offsets).pin_memory().to(dev, non_blocking=True)
-        scan_of_pair = torch.from_numpy(items.astype(np.int32)).pin_memory().to(dev, non_blocking=True)
-        train = self.mode == "train"
+            offsets = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
+            clouds = np.searchsorted(used, clouds)
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
+        offsets_d = up(offsets)
+        scan_of_cloud = up(clouds.astype(np.int32))
 
         jit = (None, None, None)
         with torch.cuda.device(dev):
             if self.rng == "device":
-                rows, cand, start, _ = ops.pair_subsample(scans, offsets_d, scan_of_pair, max_rows, N, self.n_cand,
-                                                          self.radius, self.seed, step)
+                rows, cand, start, _ = ops.cloud_subsample(scans, offsets_d, scan_of_cloud, max_rows, N, self.n_cand,
+                                                           self.radius, self.seed, step)
                 hrng = _step_rng(self.seed, step)
-                params = np.stack([draw_pair_scalars(hrng, self.opt, train, N, M, S, False)[0] for _ in range(B)])
+                drawn = [self._draw(hrng, False) for _ in range(B)]
             else:
                 rows_h = np.empty((2 * B, N), np.int32)
                 cand_h = np.empty((2 * B, self.n_cand), np.int32)
                 start_h = np.empty((2 * B,), np.int32)
-                params, jpc, jsn, jnode = [], [], [], []
-                for b in range(B):                     # KittiLoader.__getitem__, item by item
-                    pc = host_scans[b]
-                    valid = np.nonzero(radius_mask(pc, self.radius))[0] if self.radius is not None else None
-                    for side in range(2):
-                        n_valid = len(valid) if valid is not None else len(pc)
-                        choice, cand_i, start_i = draw_subsample(np.random, n_valid, N, self.divisor)
-                        rows_h[2 * b + side] = valid[choice] if valid is not None else choice
-                        cand_h[2 * b + side] = cand_i
-                        start_h[2 * b + side] = start_i
-                    p, j = draw_pair_scalars(np.random, self.opt, train, N, M, S, True)
-                    params.append(p)
-                    if j is not None:
-                        jpc.append(j[0]); jsn.append(j[1]); jnode.append(j[2])
-                params = np.stack(params)
-                up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
+                drawn = []
+                for b in range(B):                     # the reference's __getitem__, item by item
+                    for c in (2 * b, 2 * b + 1):
+                        n_valid = int(lengths[c]) if drawable is None else len(drawable[c])
+                        choice, cand_h[c], start_h[c] = draw_subsample(np.random, n_valid, N, self.divisor)
+                        rows_h[c] = choice if drawable is None else drawable[c][choice]
+                    drawn.append(self._draw(np.random, True))
                 rows, cand, start = up(rows_h), up(cand_h), up(start_h)
-                if train:
-                    jit = (up(np.stack(jpc).reshape(2 * B, N, 3)), up(np.stack(jsn).reshape(2 * B, N, S)),
-                           up(np.stack(jnode).reshape(2 * B, M, 3)))
-            params_d = torch.from_numpy(params).pin_memory().to(dev, non_blocking=True)
-            pts = ops.pair_gather_candidates(scans, offsets_d, scan_of_pair, rows, cand)
+                if drawn[0][1] is not None:
+                    jit = tuple(up(np.stack([d[1][k] for d in drawn]).reshape((2 * B,) + drawn[0][1][k].shape[1:]))
+                                for k in range(3))
+            params = np.stack([d[0] for d in drawn])
+            params = up(params.reshape(-1, params.shape[-1]))
+            pts = ops.cloud_gather_candidates(scans, offsets_d, scan_of_cloud, rows, cand)
             _, nodes = ops.fps(pts, start, M, want_nodes=True)
-            out = ops.pair_augment(scans, offsets_d, scan_of_pair, rows, nodes, params_d, S, self.flags, self.seed, step,
-                                   *jit)
-        self.last = {"rows": rows, "cand": cand, "start": start, "candidates": pts, "params": params_d}
+            out = self._augment(scans, offsets_d, scan_of_cloud, rows, nodes, params, step, jit)
+        self.last = {"rows": rows, "cand": cand, "start": start, "candidates": pts, "params": params}
         return out
+
+
+class DetectorPairBuilder(_PairBuilder):
+    """Builds the nine `ModelDetector.set_input` tensors of a batch of KITTI pairs on the device.
+
+    `build(scans, offsets, items, step=None)`: scans [T, C] f32 (device, or host -- then the items' scans are uploaded),
+    offsets (n_scans+1,) int64 row offsets (host), items the scan index of every pair.  Both clouds of a pair are
+    independent subsamples of the same scan (kitti_detector_loader.py:219-220); rng="numpy" replays
+    KittiLoader.__getitem__.  See `_PairBuilder` for the two rng modes.
+    """
+
+    def __init__(self, opt, mode="train", device=None, seed=0, rng="device", divisor=3):
+        super().__init__(opt, mode, device, seed, rng, divisor)
+        r = getattr(opt, "radius_threshold", 100.0)
+        self.radius = float(r) if r < 90 else None
+
+    def _clouds(self, items):
+        items = np.asarray(items, dtype=np.int64).ravel()
+        if items.size == 0:
+            raise ValueError("no items")
+        return np.repeat(items, 2)
+
+    def _draw(self, rng, per_point):
+        return draw_pair_scalars(rng, self.opt, self.mode == "train", self.N, self.M, self.S, per_point)
+
+    def _augment(self, scans, offsets, scan_of_cloud, rows, nodes, params, step, jit):
+        return ops.pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, self.S, self.flags, self.seed, step,
+                                *jit)
+
+    def build(self, scans, offsets, items, step=None):
+        return self._build(scans, offsets, step, items)
 
 
 # ----------------------------------------------------------------------------------------------- KITTI tree
@@ -315,14 +348,74 @@ def synthetic_scan(seed, Ns, C=8):
     return a
 
 
-class KittiPairSource:
-    """Shuffled batches of KITTI detector pairs, built on the device and handed to `ModelDetector`.
+class _KittiSource:
+    """What the KITTI detector and descriptor sources share: the scans of a tree, indexed like make_dataset_kitti (so
+    `index` names the reference's sample) and loaded once into pinned host memory, or onto the device with
+    resident="device"; shuffled epochs; and the hand-over.  Iteration builds batch i+1 on a stream of its own while the
+    caller runs step i, and hands each batch over with `model.prefetch_input(..., after=event)` + `set_input()`: the
+    model's stream waits on the build's event, the host never synchronises.  Every batch is a fresh set of tensors, so
+    a batch still in use is never overwritten.  A subclass turns the scan indices of one batch into the model's inputs
+    (`_build`, called with the build stream current)."""
 
-    Scans are indexed like make_dataset_kitti (so `index` names the reference's sample) and loaded once into pinned
-    host memory, or onto the device with resident="device".  Iteration builds batch i+1 on a stream of its own while
-    the caller runs step i, and hands each batch over with `model.prefetch_input(..., after=event)` + `set_input()`:
-    the model's stream waits on the build's event, the host never synchronises.  Every batch is a fresh set of
-    tensors, so a batch still in use is never overwritten.
+    def __init__(self, root, mode, opt, builder, device, seed, resident, rng, batch_size, drop_last):
+        self.opt, self.mode = opt, mode
+        self.device = torch.device(device if device is not None else "cuda")
+        self.batch_size = int(batch_size or opt.batch_size)
+        self.drop_last = drop_last
+        _, _, self.nums, self.accs = make_dataset_kitti(root, mode)
+        n = self.accs[-1] if self.accs else 0
+        if n == 0:
+            raise ValueError("no scans under %s" % root)
+        arrs = [load_scan_npy(kitti_scan_path(root, mode, i), opt.surface_normal_len) for i in range(n)]
+        if len({a.shape[1] for a in arrs}) != 1:
+            raise ValueError("scans differ in column count")
+        self.offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrs])]).astype(np.int64)
+        scans = torch.from_numpy(np.concatenate(arrs))
+        self.scans = scans.to(self.device) if resident == "device" else scans.pin_memory()
+        self.builder = builder(opt, mode, self.device, seed, rng)
+        self.order_rng = np.random.RandomState(seed)
+        self.stream = torch.cuda.Stream(device=self.device)
+        self.step = 0
+        self.last = None                        # what the batch last yielded was built from, for inspection
+
+    def __len__(self):
+        n = len(self.offsets) - 1
+        return n // self.batch_size if self.drop_last else -(-n // self.batch_size)
+
+    def _build(self, items):
+        """-> (the model's input tensors, what `last` will say about them)."""
+        raise NotImplementedError
+
+    def _enqueue(self, items):
+        with torch.cuda.stream(self.stream):
+            out, info = self._build(items)
+            ev = torch.cuda.Event()
+            ev.record(self.stream)
+        self.step += 1
+        return out, ev, info
+
+    def batches(self):
+        """One shuffled epoch of (input tensors, ready event); batch i+1 is enqueued before batch i is yielded."""
+        perm = self.order_rng.permutation(len(self.offsets) - 1)
+        chunks = [perm[i:i + self.batch_size] for i in range(0, len(perm), self.batch_size)]
+        if self.drop_last and chunks and len(chunks[-1]) < self.batch_size:
+            chunks.pop()
+        nxt = self._enqueue(chunks[0]) if chunks else None
+        for k in range(len(chunks)):
+            out, ev, self.last = nxt
+            nxt = self._enqueue(chunks[k + 1]) if k + 1 < len(chunks) else None
+            yield out, ev
+
+    def feed(self, model):
+        """One epoch; before each yield the batch is the model's input (prefetch_input + set_input)."""
+        for out, ev in self.batches():
+            model.prefetch_input(*out, after=ev)
+            model.set_input(*out)
+            yield out
+
+
+class KittiPairSource(_KittiSource):
+    """Shuffled batches of KITTI detector pairs, built on the device and handed to `ModelDetector` (see `_KittiSource`).
 
         src = KittiPairSource(root, "train", opt)
         for epoch in range(E):
@@ -332,52 +425,7 @@ class KittiPairSource:
 
     def __init__(self, root, mode, opt, device=None, seed=0, resident="host", rng="device", batch_size=None,
                  drop_last=True):
-        self.opt, self.mode = opt, mode
-        self.device = torch.device(device if device is not None else "cuda")
-        self.batch_size = int(batch_size or opt.batch_size)
-        self.drop_last = drop_last
-        _, _, _, accs = make_dataset_kitti(root, mode)
-        n = accs[-1] if accs else 0
-        if n == 0:
-            raise ValueError("no scans under %s" % root)
-        arrs = [load_scan_npy(kitti_scan_path(root, mode, i), opt.surface_normal_len) for i in range(n)]
-        if len({a.shape[1] for a in arrs}) != 1:
-            raise ValueError("scans differ in column count")
-        self.offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrs])]).astype(np.int64)
-        scans = torch.from_numpy(np.concatenate(arrs))
-        self.scans = scans.to(self.device) if resident == "device" else scans.pin_memory()
-        self.builder = DetectorPairBuilder(opt, mode, self.device, seed, rng)
-        self.order_rng = np.random.RandomState(seed)
-        self.stream = torch.cuda.Stream(device=self.device)
-        self.step = 0
-
-    def __len__(self):
-        n = len(self.offsets) - 1
-        return n // self.batch_size if self.drop_last else -(-n // self.batch_size)
+        super().__init__(root, mode, opt, DetectorPairBuilder, device, seed, resident, rng, batch_size, drop_last)
 
     def _build(self, items):
-        with torch.cuda.stream(self.stream):
-            out = self.builder.build(self.scans, self.offsets, items, step=self.step)
-            ev = torch.cuda.Event()
-            ev.record(self.stream)
-        self.step += 1
-        return out, ev
-
-    def batches(self):
-        """One shuffled epoch of (nine tensors, ready event); batch i+1 is enqueued before batch i is yielded."""
-        perm = self.order_rng.permutation(len(self.offsets) - 1)
-        chunks = [perm[i:i + self.batch_size] for i in range(0, len(perm), self.batch_size)]
-        if self.drop_last and chunks and len(chunks[-1]) < self.batch_size:
-            chunks.pop()
-        nxt = self._build(chunks[0]) if chunks else None
-        for k in range(len(chunks)):
-            cur = nxt
-            nxt = self._build(chunks[k + 1]) if k + 1 < len(chunks) else None
-            yield cur
-
-    def feed(self, model):
-        """One epoch; before each yield the batch is the model's input (prefetch_input + set_input)."""
-        for out, ev in self.batches():
-            model.prefetch_input(*out, after=ev)
-            model.set_input(*out)
-            yield out
+        return self.builder.build(self.scans, self.offsets, items, step=self.step), None
