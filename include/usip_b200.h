@@ -76,8 +76,8 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
                  void* stream);
 
 /* Training pairs on the device (csrc/pairgen.cu): the detector's data/kitti_detector_loader.py:101-259
- * (KittiLoader.__getitem__) and the descriptor's data/kitti_descriptor_loader.py:102-347
- * (KittiDescriptorLoader.__getitem__).
+ * (KittiLoader.__getitem__) and data/modelnet_shrec_loader.py:152-275 (ModelNet_Shrec_Loader.__getitem__), and the
+ * descriptor's data/kitti_descriptor_loader.py:102-347 (KittiDescriptorLoader.__getitem__).
  * Input: a ragged batch of raw scans, scans [T, C] f32 (x, y, z, then C-3 feature columns) with row offsets (n_scans+1)
  * i64.  Clouds are numbered c = 2*pair + side (0 = src / anchor, 1 = dst / positive); scan_of_cloud (2*n_pairs) i32 names
  * the scan of every cloud.  The detector names a pair's scan twice (both sides subsample the same scan independently), the
@@ -110,7 +110,14 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *     pair's scale, the same value in both of its clouds;
  *   jitter arrays and flags as in usip_pair_augment (the transform flags only); sn = columns 3:3+S for every S
  *     (3 + S <= C).  Test mode (no USIP_PAIR_TRAIN): the rows and the nodes as they are.
- *   -> anc/pos pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M) f32. */
+ *   -> anc/pos pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M) f32.
+ * usip_modelnet_pair_augment (data/modelnet_shrec_loader.py:182-243 ModelNet_Shrec_Loader.augment, train mode only,
+ *   then transform_pc_pytorch for dst): arguments, params layout and outputs as usip_pair_augment, but
+ *   jit_pc (n_pairs, N, 3), jit_sn (n_pairs, N, 3), jit_node (n_pairs, M, 3) are PER PAIR: row i of src and of dst gets
+ *     the same jitter, although the two clouds subsample independently.  NULL: drawn on the device with Philox keyed by
+ *     the pair, N(0, 0.01^2) clipped at 0.05 for pc and sn, N(0, 0.04^2) clipped at 0.1 for nodes;
+ *   S == 3 and sn = columns 3:6 (C >= 6).  After any rotation sn is a float64 chain (rotated, jittered, times [27]);
+ *     without one it is fp32, jittered and scaled in place.  sn is never shifted.  pc and nodes: as usip_pair_augment. */
 #define USIP_PAIR_TRAIN 1
 #define USIP_PAIR_ROT_HORIZONTAL 2
 #define USIP_PAIR_ROT_3D 4
@@ -128,6 +135,12 @@ int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const i
                       const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
                       int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node, float* dst_pc,
                       float* dst_sn, float* dst_node, float* R, float* scale, float* shift, void* stream);
+int usip_modelnet_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                               const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
+                               const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags,
+                               int S, int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node,
+                               float* dst_pc, float* dst_sn, float* dst_node, float* R, float* scale, float* shift,
+                               void* stream);
 int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                            const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
                            const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,

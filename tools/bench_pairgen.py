@@ -1,12 +1,14 @@
-"""Cost of building detector training pairs (usip_b200.data.kitti_detector_loader) -- one JSON line.
+"""Cost of building detector training pairs (usip_b200.data.kitti_detector_loader, .modelnet_shrec_loader) -- one
+JSON line.
 
   * builder: ms per batch of B pairs in device mode (CUDA events), split into subsample / candidate gather + FPS /
     augment, and the augment kernel's GB/s against its compulsory bytes;
-  * reference: ms per pair of the reference's KittiLoader.__getitem__ on the host cores (only where the reference's
-    Python tree is importable; otherwise "not measured");
-  * training loop: KittiPairSource + optimize() per step against optimize() on one resident batch.
+  * reference: ms per pair of the reference's KittiLoader / ModelNet_Shrec_Loader.__getitem__ on the host cores (only
+    where the reference's Python tree is importable; otherwise "not measured");
+  * training loop: KittiPairSource / ModelNetPairSource + optimize() per step against optimize() on one resident batch.
 
-    python tools/bench_pairgen.py [--pairs 8] [--scan-rows 20480] [--N 16384] [--M 512] [--iters 50] [--out FILE]
+    python tools/bench_pairgen.py [--dataset kitti] [--pairs 8] [--scan-rows 20480] [--N 16384] [--M 512] [--out FILE]
+    python tools/bench_pairgen.py --dataset modelnet    # defaults B=24, 10000-row objects, N=5000, M=512 (configs[1])
     python tools/bench_pairgen.py --reference-only      # host timing of the reference loader alone
 """
 import argparse
@@ -25,12 +27,36 @@ sys.path.insert(0, ROOT)
 
 from usip_b200 import ops  # noqa: E402
 from usip_b200.data import kitti_detector_loader as kdl  # noqa: E402
+from usip_b200.data import modelnet_shrec_loader as mnl  # noqa: E402
+
+# per dataset: (pairs, scan rows, N, M), S, the builder, the source and the model's configuration
+DEFAULTS = {"kitti": (8, 20480, 16384, 512), "modelnet": (24, 10000, 5000, 512)}
+MN_SHAPES = ("airplane", "night_stand", "cup")
 
 
 def kitti_opt(N, M, B, device):
     from tests.util_gpu import make_opt
     return make_opt(input_pc_num=N, node_num=M, batch_size=B, surface_normal_len=4, rot_horizontal=True, rot_3d=False,
                     rot_perturbation=False, translation_perturbation=False, radius_threshold=100.0, device=device)
+
+
+def modelnet_opt(N, M, B, device):
+    """modelnet/options_detector.py: rot_3d only, S=3, Kn=32, scene 'object'."""
+    from tests.util_gpu import make_opt
+    return make_opt(dataset="modelnet", classes=40, input_pc_num=N, node_num=M, batch_size=B, surface_normal_len=3,
+                    node_knn_k_1=32, scene="object", loss_sigma_lower_bound=1e-4, keypoint_on_pc_alpha=1.0,
+                    rot_horizontal=False, rot_3d=True, rot_perturbation=False, translation_perturbation=False,
+                    device=device)
+
+
+def setup(a, dev):
+    """-> (S, opt, builder class, scan generator, augment call(scans, off, sp, rows, nodes, params, flags))."""
+    if a.dataset == "modelnet":
+        aug = lambda *x: ops.modelnet_pair_augment(*x, 1, 0)
+        return 3, modelnet_opt(a.N, a.M, a.pairs, dev), mnl.ModelNetPairBuilder, mnl.synthetic_object, aug
+    aug = lambda sc, off, sp, rows, nodes, params, flags: ops.pair_augment(sc, off, sp, rows, nodes, params, 4, flags,
+                                                                           1, 0)
+    return 4, kitti_opt(a.N, a.M, a.pairs, dev), kdl.DetectorPairBuilder, kdl.synthetic_scan, aug
 
 
 def event_ms(fn, iters):
@@ -44,11 +70,12 @@ def event_ms(fn, iters):
 
 
 def bench_builder(a, dev):
-    B, N, M, S, C = a.pairs, a.N, a.M, 4, 8
-    arrs = [kdl.synthetic_scan(100 + i, a.scan_rows) for i in range(B)]
+    B, N, M = a.pairs, a.N, a.M
+    S, opt, builder, scan, augment = setup(a, dev)
+    arrs = [scan(100 + i, a.scan_rows) for i in range(B)]
     off = np.concatenate([[0], np.cumsum([len(x) for x in arrs])]).astype(np.int64)
     scans = torch.from_numpy(np.concatenate(arrs)).to(dev)
-    b = kdl.DetectorPairBuilder(kitti_opt(N, M, B, dev), "train", dev, seed=1)
+    b = builder(opt, "train", dev, seed=1)
     items = list(range(B))
     for s in range(5):
         b.build(scans, off, items, step=s)
@@ -64,8 +91,7 @@ def bench_builder(a, dev):
                                    a.iters)
     res["gather_fps_ms"] = event_ms(lambda: ops.fps(ops.cloud_gather_candidates(scans, off_d, sp, rows, cand), start,
                                                     M), a.iters)
-    res["augment_ms"] = event_ms(lambda: ops.pair_augment(scans, off_d, sp, rows, nodes, params, S, b.flags, 1, 0),
-                                 a.iters)
+    res["augment_ms"] = event_ms(lambda: augment(scans, off_d, sp, rows, nodes, params, b.flags), a.iters)
     # compulsory bytes of the augment kernel: row ids, the used scan columns and the nodes in; the nine outputs out
     nbytes = 2 * B * (N * 4 + N * (3 + S) * 4 + 3 * M * 4) + 2 * B * ((3 + S) * N + 3 * M) * 4 + B * 13 * 4
     res["augment_gbs"] = nbytes / (res["augment_ms"] * 1e-3) / 1e9
@@ -78,12 +104,17 @@ def bench_training_loop(a, dev):
     from tests.util_gpu import load_params
     from usip_b200.models.keypoint_detector import ModelDetector
     B, N, M = a.pairs, a.N, a.M
-    opt = kitti_opt(N, M, B, dev)
+    S, opt, _, _, _ = setup(a, dev)
     with tempfile.TemporaryDirectory() as root:
-        kdl.write_synthetic_kitti(root, [B * a.loop_batches] + [0] * 10, a.scan_rows, seed=5)
-        src = kdl.KittiPairSource(root, "train", opt, dev, seed=2)
+        if a.dataset == "modelnet":
+            mnl.write_synthetic_modelnet(root, MN_SHAPES, -(-B * a.loop_batches // len(MN_SHAPES)), 0, a.scan_rows,
+                                         seed=5)
+            src = mnl.ModelNetPairSource(root, "train", opt, dev, seed=2)
+        else:
+            kdl.write_synthetic_kitti(root, [B * a.loop_batches] + [0] * 10, a.scan_rows, seed=5)
+            src = kdl.KittiPairSource(root, "train", opt, dev, seed=2)
         md = ModelDetector(opt)
-        load_params(md.detector, orc.init_detector_params(S=4, seed=1, randomize_bn=True))
+        load_params(md.detector, orc.init_detector_params(S=S, seed=1, randomize_bn=True))
         for _ in range(2):                                        # warm-up: graph capture, allocator
             for _ in src.feed(md):
                 md.optimize(epoch=0)
@@ -109,22 +140,31 @@ def bench_training_loop(a, dev):
 
 
 def bench_reference(a):
-    """KittiLoader.__getitem__ of the reference on the host, from a staged synthetic tree (N, M as configured)."""
+    """KittiLoader / ModelNet_Shrec_Loader.__getitem__ of the reference on the host, from a staged synthetic tree (N, M
+    as configured)."""
+    modelnet = a.dataset == "modelnet"
     try:
         import importlib
         from oracle import ref_shim
         if not ref_shim.reference_available():
             return None
         ref_shim.install(use_ref_ext=False)
-        kl = importlib.import_module("data.kitti_detector_loader")
+        kl = importlib.import_module("data.modelnet_shrec_loader" if modelnet else "data.kitti_detector_loader")
     except Exception as e:                                          # the reference tree is optional
         print("[bench_pairgen] reference loader not importable: %s" % e, file=sys.stderr)
         return None
-    opt = ref_shim.make_opt(input_pc_num=a.N, node_num=a.M, surface_normal_len=4, rot_horizontal=True,
-                            radius_threshold=100.0, translation_perturbation=False, rot_perturbation=False)
     with tempfile.TemporaryDirectory() as root:
-        kdl.write_synthetic_kitti(root, [a.ref_items] + [0] * 10, a.scan_rows, seed=5)
-        loader = kl.KittiLoader(root, "train", opt)
+        if modelnet:
+            opt = ref_shim.make_opt(dataset="modelnet", classes=40, input_pc_num=a.N, node_num=a.M,
+                                    surface_normal_len=3, rot_horizontal=False, rot_3d=True, rot_perturbation=False,
+                                    translation_perturbation=False)
+            mnl.write_synthetic_modelnet(root, MN_SHAPES, -(-a.ref_items // len(MN_SHAPES)), 0, a.scan_rows, seed=5)
+            loader = kl.ModelNet_Shrec_Loader(root, "train", opt)
+        else:
+            opt = ref_shim.make_opt(input_pc_num=a.N, node_num=a.M, surface_normal_len=4, rot_horizontal=True,
+                                    radius_threshold=100.0, translation_perturbation=False, rot_perturbation=False)
+            kdl.write_synthetic_kitti(root, [a.ref_items] + [0] * 10, a.scan_rows, seed=5)
+            loader = kl.KittiLoader(root, "train", opt)
         np.random.seed(0)
         loader[0]
         t0 = time.perf_counter()
@@ -145,10 +185,11 @@ def gpu_info():
 
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--pairs", type=int, default=8)
-    p.add_argument("--scan-rows", type=int, default=20480)
-    p.add_argument("--N", type=int, default=16384)
-    p.add_argument("--M", type=int, default=512)
+    p.add_argument("--dataset", choices=sorted(DEFAULTS), default="kitti")
+    p.add_argument("--pairs", type=int, default=None)
+    p.add_argument("--scan-rows", type=int, default=None)
+    p.add_argument("--N", type=int, default=None)
+    p.add_argument("--M", type=int, default=None)
     p.add_argument("--iters", type=int, default=50)
     p.add_argument("--loop-batches", type=int, default=4)
     p.add_argument("--loop-epochs", type=int, default=5)
@@ -156,7 +197,10 @@ def main():
     p.add_argument("--reference-only", action="store_true")
     p.add_argument("--out", default=None)
     a = p.parse_args()
-    res = {"pairs": a.pairs, "scan_rows": a.scan_rows, "N": a.N, "M": a.M}
+    for k, v in zip(("pairs", "scan_rows", "N", "M"), DEFAULTS[a.dataset]):
+        if getattr(a, k) is None:
+            setattr(a, k, v)
+    res = {"dataset": a.dataset, "pairs": a.pairs, "scan_rows": a.scan_rows, "N": a.N, "M": a.M}
     if not a.reference_only:
         if not torch.cuda.is_available():
             raise SystemExit("bench_pairgen needs a CUDA device")

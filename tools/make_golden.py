@@ -424,6 +424,47 @@ def golden_descpairs(ref):
     print("descriptor_pairs.npz", os.path.getsize(os.path.join(OUT, "descriptor_pairs.npz")) // 1024, "KB")
 
 
+# data/modelnet_shrec_loader.py ModelNet_Shrec_Loader.__getitem__ (dataset 'modelnet') on a synthetic ModelNet tree
+# (usip_b200.data.modelnet_shrec_loader.write_synthetic_modelnet): every object (MN_ROWS, 6) float32.  One case builds two
+# items in a row from one seed, so a batch of two pairs with its per-pair jitter is pinned too.
+MN_SHAPES, MN_TRAIN, MN_TEST, MN_ROWS, MN_TREE_SEED, MN_N, MN_M = ("airplane", "night_stand", "cup"), 2, 1, 2000, 7300, 1000, 64
+MN_CASES = {        # name: (mode, items, np seed, rot_horizontal, rot_3d, rot_perturbation, translation)
+    "rot3d": ("train", [4, 1], 31, 0, 1, 0, 0),                 # modelnet/options_detector.py defaults
+    "horizontal": ("train", [2], 32, 1, 0, 0, 1),
+    "allrot": ("train", [5], 33, 1, 1, 1, 1),                   # the transform drops the perturbation
+    "norot": ("train", [0], 34, 0, 0, 0, 1),                    # pc and sn stay float32
+    "test": ("test", [2], 35, 0, 1, 0, 0),
+}
+
+
+def golden_modelnet_pairs(ref):
+    import importlib
+    import tempfile
+    from usip_b200.data.modelnet_shrec_loader import write_synthetic_modelnet
+    ml = importlib.import_module("data.modelnet_shrec_loader")
+    out = {"tree/shapes": np.array(MN_SHAPES), "tree/counts": np.array([MN_TRAIN, MN_TEST]),
+           "tree/rows": np.int64(MN_ROWS), "tree/seed": np.int64(MN_TREE_SEED), "N": np.int64(MN_N), "M": np.int64(MN_M)}
+    keys = ("src_pc", "src_sn", "src_node", "dst_pc", "dst_sn", "dst_node", "R", "scale", "shift")
+    with tempfile.TemporaryDirectory() as root:
+        write_synthetic_modelnet(root, MN_SHAPES, MN_TRAIN, MN_TEST, MN_ROWS, seed=MN_TREE_SEED)
+        for name, (mode, items, seed, rh, r3, rp, tp) in MN_CASES.items():
+            opt = ref_shim.make_opt(dataset="modelnet", classes=40, input_pc_num=MN_N, node_num=MN_M,
+                                    surface_normal_len=3, rot_horizontal=bool(rh), rot_3d=bool(r3),
+                                    rot_perturbation=bool(rp), translation_perturbation=bool(tp))
+            loader = ml.ModelNet_Shrec_Loader(root, mode, opt)
+            np.random.seed(seed)
+            res = [loader[i] for i in items]
+            out[name + "/case"] = np.array([seed, rh, r3, rp, tp], dtype=np.int64)
+            out[name + "/items"] = np.array(items, dtype=np.int64)
+            out[name + "/mode"] = np.array(mode)
+            for k, vals in zip(keys, zip(*res)):
+                out[name + "/" + k] = np.stack([np.asarray(v.numpy() if torch.is_tensor(v) else v, dtype=np.float32)
+                                                for v in vals])
+            print("modelnet_pairs", name, {k: out[name + "/" + k].shape for k in keys})
+    np.savez_compressed(os.path.join(OUT, "modelnet_pairs.npz"), **out)
+    print("modelnet_pairs.npz", os.path.getsize(os.path.join(OUT, "modelnet_pairs.npz")) // 1024, "KB")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)

@@ -1,6 +1,7 @@
 // pairgen.cu -- device-side construction of the detector's training pairs (SURVEY section 8 f-2, completed): the random
 // subsampling of data/kitti_detector_loader.py:118-145 (KittiLoader.get_instance_unaugmented_np), the augmentation of
-// :149-216 (KittiLoader.augment) and the dst transform of data/augmentation.py:199-248 (transform_pc_pytorch).
+// :149-216 (KittiLoader.augment) and the dst transform of data/augmentation.py:199-248 (transform_pc_pytorch); the
+// augmentation of data/modelnet_shrec_loader.py:182-243 (ModelNet_Shrec_Loader.augment, usip_modelnet_pair_augment).
 //
 // Randomness: per-pair scalars (angles, rotation matrices, scale, shifts) are drawn on the host and arrive as one
 // `params` block per pair (usip_pair_augment).  Per-point randomness is either uploaded (the caller replays numpy's
@@ -249,9 +250,10 @@ constexpr int PG_MAX_S = 8;
 // Flags: USIP_PAIR_ROT_HORIZONTAL << r is rotation r.
 constexpr int PG_ANY_ROT = USIP_PAIR_ROT_HORIZONTAL | USIP_PAIR_ROT_3D | USIP_PAIR_ROT_PERTURBATION;
 
-// clipped N(0, 0.04^2) jitter of one point or node (pc and nodes use the same law): uploaded, or Philox
+// N(0, sigma^2) jitter clipped at +-clip of one point, normal or node: uploaded (row `at` of jit), or Philox keyed by
+// (c, i, purpose).  The KITTI loaders jitter pc and nodes with sigma 0.04, clip 0.12; ModelNet's laws differ.
 __device__ __forceinline__ void pg_jitter_xyz(const double* jit, int64_t at, uint64_t seed, uint64_t step, int c, int i,
-                                              int purpose, double j[4]) {
+                                              int purpose, double sigma, double clip, double j[4]) {
   if (jit) {
     const double* q = jit + at * 3;
     j[0] = q[0]; j[1] = q[1]; j[2] = q[2];
@@ -259,7 +261,7 @@ __device__ __forceinline__ void pg_jitter_xyz(const double* jit, int64_t at, uin
     const uint4 u = pg_random(seed, step, c, i, purpose, 0);
     pg_normal2(u.x, u.y, j[0], j[1]); pg_normal2(u.z, u.w, j[2], j[3]);
 #pragma unroll
-    for (int k = 0; k < 3; ++k) j[k] = pg_clip(0.04 * j[k], 0.12);
+    for (int k = 0; k < 3; ++k) j[k] = pg_clip(sigma * j[k], clip);
   }
 }
 
@@ -328,6 +330,15 @@ __device__ __forceinline__ void pg_augment_node(int flags, const double* P, doub
   x = (float)X; y = (float)Y; z = (float)Z;
 }
 
+// transform_pc_pytorch (augmentation.py:231-245) of one dst point or node: the fp32 R as column vectors, then the fp32
+// scale and shift.  RT = the transform's R in fp32, P the pair's params block.  sn is only rotated (pg_colvec alone).
+__device__ __forceinline__ void pg_dst_transform(const float* RT, const double* P, float& x, float& y, float& z) {
+  pg_colvec(x, y, z, RT);
+  const float sc = (float)P[43];                   // float32 tensor * Python float
+  x = __fmul_rn(x, sc); y = __fmul_rn(y, sc); z = __fmul_rn(z, sc);
+  x = __fadd_rn(x, (float)P[40]); y = __fadd_rn(y, (float)P[41]); z = __fadd_rn(z, (float)P[42]);
+}
+
 __global__ void __launch_bounds__(PG_AUG_THREADS)
 pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
                     const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
@@ -360,18 +371,15 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
     for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[sn_col + k] : 0.f;
     if (train) {                                   // KittiLoader.augment, :182-212
       double j[4];
-      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, j);
+      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, 0.04, 0.12, j);
       pg_augment_point(flags, P, P[27], j, S, x, y, z, sn);
       pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, sn);
     }
     float* opc = side ? dst_pc : src_pc;
     float* osn = side ? dst_sn : src_sn;
     if (side == 1) {                               // transform_pc_pytorch, fp32, column vectors
-      pg_colvec(x, y, z, RT);
+      pg_dst_transform(RT, P, x, y, z);
       if (S >= 3) pg_colvec(sn[0], sn[1], sn[2], RT);
-      const float sc = (float)P[43];
-      x = __fmul_rn(x, sc); y = __fmul_rn(y, sc); z = __fmul_rn(z, sc);
-      x = __fadd_rn(x, (float)P[40]); y = __fadd_rn(y, (float)P[41]); z = __fadd_rn(z, (float)P[42]);
     }
     opc[((int64_t)b * 3 + 0) * N + i] = x;
     opc[((int64_t)b * 3 + 1) * N + i] = y;
@@ -386,19 +394,90 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
     float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
     if (train) {
       double j[4];
-      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, j);
+      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, 0.04, 0.12, j);
       pg_augment_node(flags, P, P[27], j, x, y, z);
     }
     float* ond = side ? dst_node : src_node;
-    if (side == 1) {
-      pg_colvec(x, y, z, RT);
-      const float sc = (float)P[43];
-      x = __fmul_rn(x, sc); y = __fmul_rn(y, sc); z = __fmul_rn(z, sc);
-      x = __fadd_rn(x, (float)P[40]); y = __fadd_rn(y, (float)P[41]); z = __fadd_rn(z, (float)P[42]);
-    }
+    if (side == 1) pg_dst_transform(RT, P, x, y, z);
     ond[((int64_t)b * 3 + 0) * M + i] = x;
     ond[((int64_t)b * 3 + 1) * M + i] = y;
     ond[((int64_t)b * 3 + 2) * M + i] = z;
+  }
+}
+
+// ModelNet sn (modelnet_shrec_loader.py:213-233): `sn_np = atomic_rotate(sn_np, .)` builds a new float64 array, so
+// after any rotation sn stays float64 through jitter and scale (the node's chain without the shift); without one it is
+// still the float32 slice, jittered in place and scaled in fp32.  sn is never shifted.
+__device__ __forceinline__ void pg_modelnet_sn(int flags, const double* P, double sc, const double* j, float& x,
+                                               float& y, float& z) {
+  if (flags & PG_ANY_ROT) {
+    pg_augment_node(flags & ~USIP_PAIR_TRANSLATION, P, sc, j, x, y, z);
+  } else {
+    x = (float)__dadd_rn((double)x, j[0]); y = (float)__dadd_rn((double)y, j[1]);
+    z = (float)__dadd_rn((double)z, j[2]);
+    const float scf = (float)sc;
+    x = __fmul_rn(x, scf); y = __fmul_rn(y, scf); z = __fmul_rn(z, scf);
+  }
+}
+
+// ModelNet pairs (ModelNet_Shrec_Loader.augment, modelnet_shrec_loader.py:182-243, then transform_pc_pytorch for dst).
+// Both clouds of pair b subsample the same file independently but read ONE draw of every jitter array: row i of src and
+// of dst gets the same numbers (jit_* are per pair, and Philox is keyed by b, not by the cloud).  pc and nodes follow
+// the KITTI arithmetic with ModelNet's jitter laws; sn = columns 3:6, see pg_modelnet_sn.
+__global__ void __launch_bounds__(PG_AUG_THREADS)
+modelnet_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
+                             const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
+                             const float* __restrict__ nodes, const double* __restrict__ params,
+                             const double* __restrict__ jit_pc, const double* __restrict__ jit_sn,
+                             const double* __restrict__ jit_node, uint64_t seed, uint64_t step, int flags, int N, int M,
+                             float* __restrict__ src_pc, float* __restrict__ src_sn, float* __restrict__ src_node,
+                             float* __restrict__ dst_pc, float* __restrict__ dst_sn, float* __restrict__ dst_node,
+                             float* __restrict__ R_out, float* __restrict__ scale_out, float* __restrict__ shift_out) {
+  const int c = blockIdx.y, b = c >> 1, side = c & 1;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const double* P = params + (int64_t)b * PG_PARAM_STRIDE;
+  const bool train = flags & USIP_PAIR_TRAIN;
+  float RT[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) RT[k] = (float)P[31 + k];
+
+  if (side == 1 && blockIdx.x == 0) {
+    if (threadIdx.x < 9) R_out[b * 9 + threadIdx.x] = RT[threadIdx.x];
+    else if (threadIdx.x == 9) scale_out[b] = (float)P[43];
+    else if (threadIdx.x < 13) shift_out[b * 3 + threadIdx.x - 10] = (float)P[40 + threadIdx.x - 10];
+  }
+
+  if (i < N) {
+    const float* p = scans + (offsets[scan_of_cloud[c]] + rows[(int64_t)c * N + i]) * C;
+    float x = p[0], y = p[1], z = p[2], nx = p[3], ny = p[4], nz = p[5];
+    if (train) {                                   // ModelNet_Shrec_Loader.augment, :182-243
+      double j[4];
+      pg_jitter_xyz(jit_pc, (int64_t)b * N + i, seed, step, b, i, PURPOSE_JIT_PC, 0.01, 0.05, j);
+      pg_augment_point(flags, P, P[27], j, 0, x, y, z, nullptr);
+      pg_jitter_xyz(jit_sn, (int64_t)b * N + i, seed, step, b, i, PURPOSE_JIT_SN, 0.01, 0.05, j);
+      pg_modelnet_sn(flags, P, P[27], j, nx, ny, nz);
+    }
+    if (side == 1) {
+      pg_dst_transform(RT, P, x, y, z);
+      pg_colvec(nx, ny, nz, RT);
+    }
+    float* opc = (side ? dst_pc : src_pc) + (int64_t)b * 3 * N;
+    float* osn = (side ? dst_sn : src_sn) + (int64_t)b * 3 * N;
+    opc[i] = x; opc[N + i] = y; opc[2 * N + i] = z;
+    osn[i] = nx; osn[N + i] = ny; osn[2 * N + i] = nz;
+  }
+
+  if (i < M) {
+    const float* nd = nodes + (int64_t)c * 3 * M;
+    float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
+    if (train) {
+      double j[4];
+      pg_jitter_xyz(jit_node, (int64_t)b * M + i, seed, step, b, i, PURPOSE_JIT_NODE, 0.04, 0.1, j);
+      pg_augment_node(flags, P, P[27], j, x, y, z);
+    }
+    if (side == 1) pg_dst_transform(RT, P, x, y, z);
+    float* ond = (side ? dst_node : src_node) + (int64_t)b * 3 * M;
+    ond[i] = x; ond[M + i] = y; ond[2 * M + i] = z;
   }
 }
 
@@ -426,7 +505,7 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
     for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[3 + k] : 0.f;
     if (train) {
       double j[4];
-      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, j);
+      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, 0.04, 0.12, j);
       pg_augment_point(flags, P, P[27], j, S, x, y, z, sn);
       pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, sn);
     }
@@ -445,7 +524,7 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
     float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
     if (train) {
       double j[4];
-      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, j);
+      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, 0.04, 0.12, j);
       pg_augment_node(flags, P, P[27], j, x, y, z);
     }
     float* ond = side ? pos_node : anc_node;
@@ -534,4 +613,23 @@ extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offse
       scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, sn_col, N,
       M, src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, R, scale, shift);
   return check_launch("pair_augment_kernel");
+}
+
+extern "C" int usip_modelnet_pair_augment(const float* scans, int C, const int64_t* offsets,
+                                          const int32_t* scan_of_cloud, const int32_t* rows, const float* nodes,
+                                          const double* params, const double* jit_pc, const double* jit_sn,
+                                          const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
+                                          int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node,
+                                          float* dst_pc, float* dst_sn, float* dst_node, float* R, float* scale,
+                                          float* shift, void* stream) {
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes && params, "modelnet_pair_augment: null input");
+  USIP_REQUIRE(src_pc && src_sn && src_node && dst_pc && dst_sn && dst_node && R && scale && shift,
+               "modelnet_pair_augment: null output");
+  USIP_REQUIRE(S == 3 && C >= 6, "modelnet_pair_augment: sn is columns 3:6 (S == 3, C >= 6)");
+  USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "modelnet_pair_augment: bad sizes");
+  dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
+  modelnet_pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
+      scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, N, M, src_pc,
+      src_sn, src_node, dst_pc, dst_sn, dst_node, R, scale, shift);
+  return check_launch("modelnet_pair_augment_kernel");
 }

@@ -4,8 +4,9 @@
 whole training batch of `KittiLoader.__getitem__` (:218-259) on the device -- random subsampling, FPS nodes,
 augmentation and the dst transform -- and `KittiPairSource` feeds such batches to `ModelDetector` from a KITTI tree.
 The reference runs all of this per pair in DataLoader workers: serial numpy, more host time per pair than a whole
-training step of this repository.  Only the KITTI loaders are covered (the descriptor's builds on the bases here); the
-Oxford / ModelNet / SceneNN / Match3D loaders differ in the candidate divisor (a parameter here) and in using two scans.
+training step of this repository.  The KITTI loaders and the ModelNet detector loader (modelnet_shrec_loader.py) build
+on the bases here; the Oxford / SceneNN / Match3D loaders differ in the candidate divisor (a parameter here) and in
+using two scans.
 """
 import os
 
@@ -176,7 +177,8 @@ class _PairBuilder:
         """Reject scans too short for the subclass's loader (every scan here has at least one row)."""
 
     def _draw(self, rng, per_point):
-        """One pair's scalars -> (params block, jitter (pc (2,N,3), sn (2,N,S), node (2,M,3)) or None)."""
+        """One pair's scalars -> (params block, jitter (pc, sn, node) or None: per cloud (2, N, 3), (2, N, S), (2, M, 3),
+        or per pair (N, 3), (N, 3), (M, 3))."""
         raise NotImplementedError
 
     def _augment(self, scans, offsets, scan_of_cloud, rows, nodes, params, step, jit):
@@ -240,8 +242,8 @@ class _PairBuilder:
                         rows_h[c] = choice if drawable is None else drawable[c][choice]
                     drawn.append(self._draw(np.random, True))
                 rows, cand, start = up(rows_h), up(cand_h), up(start_h)
-                if drawn[0][1] is not None:
-                    jit = tuple(up(np.stack([d[1][k] for d in drawn]).reshape((2 * B,) + drawn[0][1][k].shape[1:]))
+                if drawn[0][1] is not None:            # per cloud (2, n, k) -> (2B, n, k); per pair (n, k) -> (B, n, k)
+                    jit = tuple(up(np.stack([d[1][k] for d in drawn]).reshape((-1,) + drawn[0][1][k].shape[-2:]))
                                 for k in range(3))
             params = np.stack([d[0] for d in drawn])
             params = up(params.reshape(-1, params.shape[-1]))
@@ -348,25 +350,21 @@ def synthetic_scan(seed, Ns, C=8):
     return a
 
 
-class _KittiSource:
-    """What the KITTI detector and descriptor sources share: the scans of a tree, indexed like make_dataset_kitti (so
-    `index` names the reference's sample) and loaded once into pinned host memory, or onto the device with
-    resident="device"; shuffled epochs; and the hand-over.  Iteration builds batch i+1 on a stream of its own while the
-    caller runs step i, and hands each batch over with `model.prefetch_input(..., after=event)` + `set_input()`: the
-    model's stream waits on the build's event, the host never synchronises.  Every batch is a fresh set of tensors, so
-    a batch still in use is never overwritten.  A subclass turns the scan indices of one batch into the model's inputs
-    (`_build`, called with the build stream current)."""
+class _ScanSource:
+    """What every device-built pair source shares, whatever its tree: a list of `.npy` scans (`paths[i]` is the scan of
+    item i) loaded once into pinned host memory, or onto the device with resident="device"; shuffled epochs; and the
+    hand-over.  Iteration builds batch i+1 on a stream of its own while the caller runs step i, and hands each batch over
+    with `model.prefetch_input(..., after=event)` + `set_input()`: the model's stream waits on the build's event, the
+    host never synchronises.  Every batch is a fresh set of tensors, so a batch still in use is never overwritten.  A
+    subclass turns the item indices of one batch into the model's inputs (`_build`, called with the build stream
+    current)."""
 
-    def __init__(self, root, mode, opt, builder, device, seed, resident, rng, batch_size, drop_last):
+    def __init__(self, paths, mode, opt, builder, device, seed, resident, rng, batch_size, drop_last):
         self.opt, self.mode = opt, mode
         self.device = torch.device(device if device is not None else "cuda")
         self.batch_size = int(batch_size or opt.batch_size)
         self.drop_last = drop_last
-        _, _, self.nums, self.accs = make_dataset_kitti(root, mode)
-        n = self.accs[-1] if self.accs else 0
-        if n == 0:
-            raise ValueError("no scans under %s" % root)
-        arrs = [load_scan_npy(kitti_scan_path(root, mode, i), opt.surface_normal_len) for i in range(n)]
+        arrs = [load_scan_npy(p, opt.surface_normal_len) for p in paths]
         if len({a.shape[1] for a in arrs}) != 1:
             raise ValueError("scans differ in column count")
         self.offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrs])]).astype(np.int64)
@@ -414,8 +412,21 @@ class _KittiSource:
             yield out
 
 
+class _KittiSource(_ScanSource):
+    """The scans of a KITTI tree for the detector and descriptor sources, indexed like make_dataset_kitti (so `index`
+    names the reference's sample).  See `_ScanSource`."""
+
+    def __init__(self, root, mode, opt, builder, device, seed, resident, rng, batch_size, drop_last):
+        _, _, self.nums, self.accs = make_dataset_kitti(root, mode)
+        n = self.accs[-1] if self.accs else 0
+        if n == 0:
+            raise ValueError("no scans under %s" % root)
+        super().__init__([kitti_scan_path(root, mode, i) for i in range(n)], mode, opt, builder, device, seed, resident,
+                         rng, batch_size, drop_last)
+
+
 class KittiPairSource(_KittiSource):
-    """Shuffled batches of KITTI detector pairs, built on the device and handed to `ModelDetector` (see `_KittiSource`).
+    """Shuffled batches of KITTI detector pairs, built on the device and handed to `ModelDetector` (see `_ScanSource`).
 
         src = KittiPairSource(root, "train", opt)
         for epoch in range(E):

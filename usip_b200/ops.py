@@ -209,6 +209,28 @@ def pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, S, flags, s
     return out
 
 
+def modelnet_pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, flags, seed=0, step=0, jit_pc=None,
+                          jit_sn=None, jit_node=None):
+    """ModelNet detector augmentation + dst transform -> the nine ModelDetector.set_input tensors, sn = scan columns
+    3:6.  params (B, 48) f64 on the device (layout in include/usip_b200.h); jitter arrays f64 PER PAIR -- jit_pc and
+    jit_sn (B, N, 3), jit_node (B, M, 3), shared by the pair's two clouds -- or None (drawn on the device from
+    (seed, step))."""
+    _req_scans(scans, offsets, scan_of_cloud); _req(rows, i32, "rows"); _req(nodes, f32, "nodes")
+    _req(params, torch.float64, "params"); _req_jitter(jit_pc, jit_sn, jit_node)
+    B, N, M, dev = scan_of_cloud.shape[0] // 2, rows.shape[1], nodes.shape[2], scans.device
+    for name, j, n in (("jit_pc", jit_pc, N), ("jit_sn", jit_sn, N), ("jit_node", jit_node, M)):
+        if j is not None and tuple(j.shape) != (B, n, 3):
+            raise ValueError("%s must be (%d, %d, 3), one array per pair; got %s" % (name, B, n, tuple(j.shape)))
+    e = lambda *s: torch.empty(s, dtype=f32, device=dev)
+    out = (e(B, 3, N), e(B, 3, N), e(B, 3, M), e(B, 3, N), e(B, 3, N), e(B, 3, M), e(B, 3, 3), e(B), e(B, 3, 1))
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_modelnet_pair_augment(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows), _p(nodes), _p(params), _p(jit_pc),
+            _p(jit_sn), _p(jit_node), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), int(flags), 3, B, N, M,
+            *[_p(t) for t in out], _stream()), "usip_modelnet_pair_augment")
+    return out
+
+
 def desc_pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, S, flags, seed=0, step=0, jit_pc=None,
                       jit_sn=None, jit_node=None):
     """Descriptor augmentation -> (anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node).  params (2B, 32) f64 per cloud
