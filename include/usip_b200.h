@@ -99,7 +99,7 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *   rows as above, nodes (2*n_pairs, 3, M) f32 = the FPS nodes (usip_fps_f32 out_nodes);
  *   params (n_pairs, 48) f64 per pair: [0:9] horizontal, [9:18] 3-d and [18:27] perturbation rotation matrices (row
  *     major, applied as data @ R in float64), [27] augmentation scale, [28:31] augmentation shift, [31:40] the transform's
- *     R (fp32 values), [40:43] its shift, [43] its scale;
+ *     R (fp32 values), [40:43] its shift, [43] its scale, [44] the Oxford height scale (USIP_PAIR_HEIGHT_SCALE);
  *   jit_pc (2*n_pairs, N, 3), jit_sn (2*n_pairs, N, S), jit_node (2*n_pairs, M, 3) f64 clipped jitter, each NULL to draw
  *     it on the device (N(0, 0.04^2) clipped at 0.12 for pc / node, N(0, 0.01^2) clipped at 0.05 for sn);
  *   flags: USIP_PAIR_* below.  sn = columns 3:3+S of the scan, or the last column when S == 1.
@@ -117,12 +117,23 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *     the same jitter, although the two clouds subsample independently.  NULL: drawn on the device with Philox keyed by
  *     the pair, N(0, 0.01^2) clipped at 0.05 for pc and sn, N(0, 0.04^2) clipped at 0.1 for nodes;
  *   S == 3 and sn = columns 3:6 (C >= 6).  After any rotation sn is a float64 chain (rotated, jittered, times [27]);
- *     without one it is fp32, jittered and scaled in place.  sn is never shifted.  pc and nodes: as usip_pair_augment. */
+ *     without one it is fp32, jittered and scaled in place.  sn is never shifted.  pc and nodes: as usip_pair_augment.
+ * Oxford scans (data/oxford_detector_loader.py, oxford_descriptor_loader.py) are ENU, z up.  USIP_PAIR_ENU_TO_CAM makes
+ *   usip_pair_augment and usip_desc_pair_augment first map every row and node to the camera frame, (x, y, z) ->
+ *   (x, -z, y), and sn columns 0:3 alike (requires S >= 3); then they run as above.  USIP_PAIR_HEIGHT_SCALE (detector
+ *   only, with USIP_PAIR_ENU_TO_CAM, applied in train mode only): before the frame change a row's z becomes
+ *   fl32(z * fl32(hs)), hs = params[b, 44].
+ * usip_cloud_gather_candidates_zscaled: usip_cloud_gather_candidates with z multiplied by z_scale[c] (2*n_pairs) f32 in
+ *   fp32, the height-scaled FPS input of the Oxford detector.
+ * usip_scale_channel_f32: t (B, C, L) f32 in place, t[b, k, :] *= factor in fp32 (the descriptor batch's height
+ *   scaling, oxford/train_descriptor.py). */
 #define USIP_PAIR_TRAIN 1
 #define USIP_PAIR_ROT_HORIZONTAL 2
 #define USIP_PAIR_ROT_3D 4
 #define USIP_PAIR_ROT_PERTURBATION 8
 #define USIP_PAIR_TRANSLATION 16
+#define USIP_PAIR_ENU_TO_CAM 32
+#define USIP_PAIR_HEIGHT_SCALE 64
 int usip_pair_max_scan_rows(void);
 int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud, int max_rows,
                          int n_pairs, int N, int n_cand, int use_radius, double radius, uint64_t seed, uint64_t step,
@@ -130,6 +141,11 @@ int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, cons
 int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                                  const int32_t* rows, const int32_t* cand, float* out_pts, int n_pairs, int N,
                                  int n_cand, void* stream);
+int usip_cloud_gather_candidates_zscaled(const float* scans, int C, const int64_t* offsets,
+                                         const int32_t* scan_of_cloud, const int32_t* rows, const int32_t* cand,
+                                         const float* z_scale, float* out_pts, int n_pairs, int N, int n_cand,
+                                         void* stream);
+int usip_scale_channel_f32(float* t, int B, int C, int L, int k, float factor, void* stream);
 int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                       const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
                       const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,

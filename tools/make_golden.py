@@ -465,6 +465,103 @@ def golden_modelnet_pairs(ref):
     print("modelnet_pairs.npz", os.path.getsize(os.path.join(OUT, "modelnet_pairs.npz")) // 1024, "KB")
 
 
+# data/oxford_detector_loader.py OxfordLoader.__getitem__ and data/oxford_descriptor_loader.py OxfordDescriptorLoader
+# (items + default_collate + mine_negative_sample) on a synthetic Oxford tree (usip_b200.data.oxford_detector_loader.
+# write_synthetic_oxford): OX_TRAIN ENU scans along a line (positives within 2, non-negatives within 4), an invalid line
+# in train_relative.txt, OX_TEST test scans numbered 100 + 3 i; every scan (OX_ROWS, 8) float32.
+OX_TRAIN, OX_TEST, OX_ROWS, OX_TREE_SEED, OX_N, OX_M = 16, 6, 1300, 7400, 1024, 64
+OX_DESC_N = 512                                   # the descriptor's batches: 4 pairs
+OX_CASES = {        # name: (mode, item, np seed, S, rot_horizontal, rot_3d, rot_perturbation, translation, height scaling)
+    "default": ("train", 9, 41, 4, 1, 0, 0, 0, 1),              # oxford/options_detector.py defaults
+    "s3": ("train", 2, 42, 3, 1, 0, 0, 0, 1),
+    "s5": ("train", 14, 43, 5, 1, 0, 0, 0, 1),
+    "rot3d": ("train", 5, 44, 4, 0, 1, 1, 1, 1),
+    "noheight": ("train", 11, 45, 4, 1, 0, 0, 0, 0),
+    "test": ("test", 3, 46, 4, 1, 0, 0, 0, 1),
+}
+OX_DESC_CASES = {   # name: (mode, items, np / random seed, S, rot_horizontal, rot_3d, rot_perturbation, translation)
+    "train": ("train", [3, 12, 7, 0], 51, 4, 1, 0, 0, 0),
+    "noneg": ("train", [5, 6, 9, 12], 52, 5, 0, 1, 1, 1),     # anchor 2 (line 9) has no negative in this batch
+    "test": ("test", [0, 3, 1, 5], 53, 4, 1, 0, 0, 0),        # the mining runs B times
+}
+
+
+def _oxford_tree(root):
+    from usip_b200.data.oxford_detector_loader import write_synthetic_oxford
+    write_synthetic_oxford(root, OX_TRAIN, OX_ROWS, n_test=OX_TEST, seed=OX_TREE_SEED)
+    return {"tree/counts": np.array([OX_TRAIN, OX_TEST]), "tree/rows": np.int64(OX_ROWS),
+            "tree/seed": np.int64(OX_TREE_SEED), "N": np.int64(OX_N), "M": np.int64(OX_M)}
+
+
+def golden_oxford_pairs(ref):
+    import importlib
+    import tempfile
+    ol = importlib.import_module("data.oxford_detector_loader")
+    keys = ("src_pc", "src_sn", "src_node", "dst_pc", "dst_sn", "dst_node", "R", "scale", "shift")
+    with tempfile.TemporaryDirectory() as root:
+        out = _oxford_tree(root)
+        for name, (mode, index, seed, S, rh, r3, rp, tp, hsc) in OX_CASES.items():
+            opt = ref_shim.make_opt(input_pc_num=OX_N, node_num=OX_M, surface_normal_len=S, rot_horizontal=bool(rh),
+                                    rot_3d=bool(r3), rot_perturbation=bool(rp), translation_perturbation=bool(tp),
+                                    is_height_scaling=bool(hsc))
+            loader = ol.OxfordLoader(root, mode, opt)
+            np.random.seed(seed)
+            res = loader[index]
+            out[name + "/case"] = np.array([index, seed, S, rh, r3, rp, tp, hsc], dtype=np.int64)
+            out[name + "/mode"] = np.array(mode)
+            for k, v in zip(keys, res):
+                out[name + "/" + k] = np.asarray(v.numpy() if torch.is_tensor(v) else v, dtype=np.float32)
+            print("oxford_pairs", name, {k: out[name + "/" + k].shape for k in keys})
+    np.savez_compressed(os.path.join(OUT, "oxford_pairs.npz"), **out)
+    print("oxford_pairs.npz", os.path.getsize(os.path.join(OUT, "oxford_pairs.npz")) // 1024, "KB")
+
+
+def golden_oxford_descpairs(ref):
+    import importlib
+    import tempfile
+    import types
+    from torch.utils.data.dataloader import default_collate
+    if "torch._six" not in sys.modules:                    # removed from torch; the loader only imports these names
+        sys.modules["torch._six"] = types.ModuleType("torch._six")
+        sys.modules["torch._six"].__dict__.update(string_classes=str, int_classes=int,
+                                                 FileNotFoundError=FileNotFoundError)
+    dl = importlib.import_module("data.oxford_descriptor_loader")
+    keys = ("anc_pc", "anc_sn", "anc_node", "pos_pc", "pos_sn", "pos_node", "index")
+    loaded = []
+    np_load = np.load
+
+    def logging_load(path, *a, **k):                       # which scan each item and positive reads
+        loaded.append(os.path.basename(str(path)))
+        return np_load(path, *a, **k)
+    with tempfile.TemporaryDirectory() as root:
+        out = _oxford_tree(root)
+        out["N"] = np.int64(OX_DESC_N)
+        np.load = logging_load
+        try:
+            for name, (mode, items, seed, S, rh, r3, rp, tp) in OX_DESC_CASES.items():
+                opt = ref_shim.make_opt(input_pc_num=OX_DESC_N, node_num=OX_M, surface_normal_len=S,
+                                        rot_horizontal=bool(rh), rot_3d=bool(r3), rot_perturbation=bool(rp),
+                                        translation_perturbation=bool(tp))
+                loader = dl.OxfordDescriptorLoader(root, mode, opt)
+                np.random.seed(seed)
+                random.seed(seed)
+                del loaded[:]
+                batch = default_collate([loader[i] for i in items])
+                neg_idx = loader.mine_negative_sample(batch[6])
+                out[name + "/case"] = np.array([seed, S, rh, r3, rp, tp], dtype=np.int64)
+                out[name + "/items"] = np.array(items, dtype=np.int64)
+                out[name + "/mode"] = np.array(mode)
+                for k, v in zip(keys, batch):
+                    out[name + "/" + k] = v.numpy()
+                out[name + "/pos_file"] = np.array([int(f.split(".")[0]) for f in loaded[1::2]], dtype=np.int64)
+                out[name + "/neg_idx"] = neg_idx.numpy()
+                print("oxford_descpairs", name, "pos_file", out[name + "/pos_file"], "neg_idx", out[name + "/neg_idx"])
+        finally:
+            np.load = np_load
+    np.savez_compressed(os.path.join(OUT, "oxford_descpairs.npz"), **out)
+    print("oxford_descpairs.npz", os.path.getsize(os.path.join(OUT, "oxford_descpairs.npz")) // 1024, "KB")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)

@@ -70,6 +70,9 @@ SIGNATURES = {
     "usip_cloud_subsample": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_int, c_int, c_int, c_int, c_int, ctypes.c_double,
                                      ctypes.c_uint64, ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr]),
     "usip_cloud_gather_candidates": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
+    "usip_cloud_gather_candidates_zscaled": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int,
+                                                     c_int, c_ptr]),
+    "usip_scale_channel_f32": (c_int, [c_ptr, c_int, c_int, c_int, c_int, ctypes.c_float, c_ptr]),
     "usip_desc_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                        ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
                                + [c_ptr] * 6 + [c_ptr]),

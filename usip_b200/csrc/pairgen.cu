@@ -1,7 +1,8 @@
 // pairgen.cu -- device-side construction of the detector's training pairs (SURVEY section 8 f-2, completed): the random
 // subsampling of data/kitti_detector_loader.py:118-145 (KittiLoader.get_instance_unaugmented_np), the augmentation of
 // :149-216 (KittiLoader.augment) and the dst transform of data/augmentation.py:199-248 (transform_pc_pytorch); the
-// augmentation of data/modelnet_shrec_loader.py:182-243 (ModelNet_Shrec_Loader.augment, usip_modelnet_pair_augment).
+// augmentation of data/modelnet_shrec_loader.py:182-243 (ModelNet_Shrec_Loader.augment, usip_modelnet_pair_augment);
+// the ENU-to-camera frame and height scaling of the Oxford loaders (pg_enu_to_cam, usip_scale_channel_f32).
 //
 // Randomness: per-pair scalars (angles, rotation matrices, scale, shifts) are drawn on the host and arrive as one
 // `params` block per pair (usip_pair_augment).  Per-point randomness is either uploaded (the caller replays numpy's
@@ -210,16 +211,18 @@ pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __rest
   }
 }
 
-// candidate points for FPS: pts[c, j, :] = xyz of row rows[c, cand[c, j]]
+// candidate points for FPS: pts[c, j, :] = xyz of row rows[c, cand[c, j]]; with z_scale, z is fl32(z * z_scale[c])
+// (the Oxford detector's height scaling, which comes before its FPS)
 __global__ void pair_gather_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
                                    const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
-                                   const int32_t* __restrict__ cand, float* __restrict__ pts, int N, int n_cand) {
+                                   const int32_t* __restrict__ cand, const float* __restrict__ z_scale,
+                                   float* __restrict__ pts, int N, int n_cand) {
   const int c = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n_cand) return;
   const int r = rows[(int64_t)c * N + cand[(int64_t)c * n_cand + j]];
   const float* p = scans + (offsets[scan_of_cloud[c]] + r) * C;
   float* o = pts + ((int64_t)c * n_cand + j) * 3;
-  o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
+  o[0] = p[0]; o[1] = p[1]; o[2] = z_scale ? __fmul_rn(p[2], z_scale[c]) : p[2];
 }
 
 // row vector times R (numpy `data @ R`, augmentation.py:62-72), float64.  The host BLAS (numpy's dgemm) accumulates
@@ -330,6 +333,24 @@ __device__ __forceinline__ void pg_augment_node(int flags, const double* P, doub
   x = (float)X; y = (float)Y; z = (float)Z;
 }
 
+// The Oxford loaders' scans are ENU (z up).  coordinate_ENU_to_cam (augmentation.py:266-278) maps (x, y, z) to
+// (x, -z, y), and sn columns 0:3 alike (S >= 3; the other columns stay); it is exact in any precision.  Before it, the
+// detector's height scaling (oxford_detector_loader.py:188-192, train mode) multiplies pc z in place, a float32 array
+// times a Python float: fl32(z * fl32(hs)).  A node has no height step here: its FPS candidates were gathered scaled.
+// Runs on the raw row or node before any augmentation; without USIP_PAIR_ENU_TO_CAM it does nothing.
+constexpr int PG_HEIGHT_SCALED = USIP_PAIR_TRAIN | USIP_PAIR_HEIGHT_SCALE;
+
+__device__ __forceinline__ void pg_enu_to_cam(int flags, double hs, float& y, float& z, float* sn, int S) {
+  if (!(flags & USIP_PAIR_ENU_TO_CAM)) return;
+  if ((flags & PG_HEIGHT_SCALED) == PG_HEIGHT_SCALED) z = __fmul_rn(z, (float)hs);
+  const float t = y;
+  y = -z; z = t;
+  if (S >= 3) {
+    const float s1 = sn[1];
+    sn[1] = -sn[2]; sn[2] = s1;
+  }
+}
+
 // transform_pc_pytorch (augmentation.py:231-245) of one dst point or node: the fp32 R as column vectors, then the fp32
 // scale and shift.  RT = the transform's R in fp32, P the pair's params block.  sn is only rotated (pg_colvec alone).
 __device__ __forceinline__ void pg_dst_transform(const float* RT, const double* P, float& x, float& y, float& z) {
@@ -369,6 +390,7 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
     float sn[PG_MAX_S];
 #pragma unroll
     for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[sn_col + k] : 0.f;
+    pg_enu_to_cam(flags, P[44], y, z, sn, S);      // Oxford only: height scale, then the camera frame
     if (train) {                                   // KittiLoader.augment, :182-212
       double j[4];
       pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, 0.04, 0.12, j);
@@ -392,6 +414,7 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
   if (i < M) {
     const float* nd = nodes + (int64_t)c * 3 * M;
     float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
+    pg_enu_to_cam(flags & ~USIP_PAIR_HEIGHT_SCALE, 1.0, y, z, nullptr, 0);
     if (train) {
       double j[4];
       pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, 0.04, 0.12, j);
@@ -503,6 +526,7 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
     float sn[PG_MAX_S];
 #pragma unroll
     for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[3 + k] : 0.f;
+    pg_enu_to_cam(flags, 1.0, y, z, sn, S);        // Oxford only: the camera frame
     if (train) {
       double j[4];
       pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, 0.04, 0.12, j);
@@ -522,6 +546,7 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
   if (i < M) {
     const float* nd = nodes + (int64_t)c * 3 * M;
     float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
+    pg_enu_to_cam(flags, 1.0, y, z, nullptr, 0);
     if (train) {
       double j[4];
       pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, 0.04, 0.12, j);
@@ -532,6 +557,14 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
     ond[((int64_t)b * 3 + 1) * M + i] = y;
     ond[((int64_t)b * 3 + 2) * M + i] = z;
   }
+}
+
+// t[b, k, :] *= f in fp32 (torch's `t[:, k, :] *= f` with f a Python float: fl32(v * fl32(f)))
+__global__ void scale_channel_kernel(float* __restrict__ t, int C, int L, int k, float f) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L) return;
+  float* row = t + ((int64_t)blockIdx.y * C + k) * L;
+  row[i] = __fmul_rn(row[i], f);
 }
 
 }  // namespace usip
@@ -568,15 +601,37 @@ extern "C" int usip_cloud_subsample(const float* scans, int C, const int64_t* of
   return check_launch("pair_subset_kernel(candidates)");
 }
 
-extern "C" int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets,
-                                            const int32_t* scan_of_cloud, const int32_t* rows, const int32_t* cand,
-                                            float* out_pts, int n_pairs, int N, int n_cand, void* stream) {
+static int pg_gather(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                     const int32_t* rows, const int32_t* cand, const float* z_scale, float* out_pts, int n_pairs, int N,
+                     int n_cand, void* stream) {
   USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && cand && out_pts, "cloud_gather_candidates: null pointer");
   USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N, "cloud_gather_candidates: bad sizes");
   dim3 grid(cdiv(n_cand, 256), 2 * n_pairs);
-  pair_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of_cloud, rows, cand, out_pts, N,
-                                                              n_cand);
+  pair_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of_cloud, rows, cand, z_scale,
+                                                              out_pts, N, n_cand);
   return check_launch("pair_gather_kernel");
+}
+
+extern "C" int usip_cloud_gather_candidates(const float* scans, int C, const int64_t* offsets,
+                                            const int32_t* scan_of_cloud, const int32_t* rows, const int32_t* cand,
+                                            float* out_pts, int n_pairs, int N, int n_cand, void* stream) {
+  return pg_gather(scans, C, offsets, scan_of_cloud, rows, cand, nullptr, out_pts, n_pairs, N, n_cand, stream);
+}
+
+extern "C" int usip_cloud_gather_candidates_zscaled(const float* scans, int C, const int64_t* offsets,
+                                                    const int32_t* scan_of_cloud, const int32_t* rows,
+                                                    const int32_t* cand, const float* z_scale, float* out_pts,
+                                                    int n_pairs, int N, int n_cand, void* stream) {
+  USIP_REQUIRE(z_scale, "cloud_gather_candidates_zscaled: null z_scale");
+  return pg_gather(scans, C, offsets, scan_of_cloud, rows, cand, z_scale, out_pts, n_pairs, N, n_cand, stream);
+}
+
+extern "C" int usip_scale_channel_f32(float* t, int B, int C, int L, int k, float factor, void* stream) {
+  USIP_REQUIRE(t, "scale_channel: null pointer");
+  USIP_REQUIRE(B > 0 && C > 0 && L > 0 && k >= 0 && k < C && B <= 65535, "scale_channel: bad sizes");
+  dim3 grid(cdiv(L, 256), B);
+  scale_channel_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(t, C, L, k, factor);
+  return check_launch("scale_channel_kernel");
 }
 
 extern "C" int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
@@ -588,6 +643,8 @@ extern "C" int usip_desc_pair_augment(const float* scans, int C, const int64_t* 
   USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes && params, "desc_pair_augment: null input");
   USIP_REQUIRE(anc_pc && anc_sn && anc_node && pos_pc && pos_sn && pos_node, "desc_pair_augment: null output");
   USIP_REQUIRE(S >= 1 && S <= PG_MAX_S && 3 + S <= C, "desc_pair_augment: bad surface-normal length");
+  USIP_REQUIRE(!(flags & USIP_PAIR_HEIGHT_SCALE), "desc_pair_augment: no height scaling in the descriptor's clouds");
+  USIP_REQUIRE(!(flags & USIP_PAIR_ENU_TO_CAM) || S >= 3, "desc_pair_augment: the camera frame needs S >= 3");
   USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "desc_pair_augment: bad sizes");
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
   desc_pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
@@ -606,6 +663,9 @@ extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offse
   USIP_REQUIRE(src_pc && src_sn && src_node && dst_pc && dst_sn && dst_node && R && scale && shift,
                "pair_augment: null output");
   USIP_REQUIRE(S >= 1 && S <= PG_MAX_S && (S == 1 || 3 + S <= C) && C >= 4, "pair_augment: bad surface-normal length");
+  USIP_REQUIRE(!(flags & USIP_PAIR_ENU_TO_CAM) || S >= 3, "pair_augment: the camera frame needs S >= 3");
+  USIP_REQUIRE(!(flags & USIP_PAIR_HEIGHT_SCALE) || (flags & USIP_PAIR_ENU_TO_CAM),
+               "pair_augment: height scaling is part of the ENU frame step");
   USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "pair_augment: bad sizes");
   const int sn_col = S == 1 ? C - 1 : 3;           // kitti_detector_loader.py:135-139
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);

@@ -82,14 +82,15 @@ def mine_negative_sample(anc_seq, anc_pose, threshold, rng=np.random):
     return neg_idx
 
 
-def draw_desc_pair_scalars(rng, train, N, M, S, per_point):
+def draw_desc_pair_scalars(rng, train, N, M, S, per_point, scale_range=(0.9, 1.1)):
     """Scalars of KittiDescriptorLoader.augment (:205-276) for one pair, in the reference's order ->
     (params (2, 32) f64 per cloud, scale, jitter (pc (2,N,3), sn (2,N,S), node (2,M,3)) or None).
-    per_point=False skips the O(N) jitter draws (the device draws its own)."""
+    per_point=False skips the O(N) jitter draws (the device draws its own).  scale_range: the pair's scale law, KITTI's
+    by default; None draws nothing and the scale is 1.0 (OxfordDescriptorLoader.augment)."""
     p = np.zeros((2, ops.DESC_PARAM_STRIDE), dtype=np.float64)
     if not train:
         return p, 0.0, None
-    scale = rng.uniform(low=0.9, high=1.1)
+    scale = rng.uniform(low=scale_range[0], high=scale_range[1]) if scale_range is not None else 1.0
     jit = ([], [], [])
     for side in range(2):
         y_angle = rng.uniform() * 2 * np.pi

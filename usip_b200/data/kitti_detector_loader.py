@@ -4,9 +4,8 @@
 whole training batch of `KittiLoader.__getitem__` (:218-259) on the device -- random subsampling, FPS nodes,
 augmentation and the dst transform -- and `KittiPairSource` feeds such batches to `ModelDetector` from a KITTI tree.
 The reference runs all of this per pair in DataLoader workers: serial numpy, more host time per pair than a whole
-training step of this repository.  The KITTI loaders and the ModelNet detector loader (modelnet_shrec_loader.py) build
-on the bases here; the Oxford / SceneNN / Match3D loaders differ in the candidate divisor (a parameter here) and in
-using two scans.
+training step of this repository.  The KITTI loaders, the ModelNet detector loader (modelnet_shrec_loader.py) and the
+Oxford loaders (oxford_detector_loader.py, oxford_descriptor_loader.py) build on the bases here.
 """
 import os
 
@@ -77,10 +76,11 @@ def draw_subsample(rng, n_valid, N, divisor=3):
     return choice, cand, start
 
 
-def draw_pair_scalars(rng, opt, train, N, M, S, per_point):
+def draw_pair_scalars(rng, opt, train, N, M, S, per_point, scale_range=(0.9, 1.1)):
     """Scalars of augment() (:157-175, train only) and transform_pc_pytorch (augmentation.py:210-243) for one pair,
     in the reference's order -> (params (48,) f64, jitter (pc (2,N,3), sn (2,N,S), node (2,M,3)) or None).
-    per_point=False skips the O(N) jitter draws (the device draws its own)."""
+    per_point=False skips the O(N) jitter draws (the device draws its own).  scale_range: the augmentation scale's
+    uniform law, KITTI's by default (the Oxford detector's is (0.7, 1.3))."""
     p = np.zeros(ops.PAIR_PARAM_STRIDE, dtype=np.float64)
     jit = None
     if train:
@@ -91,7 +91,7 @@ def draw_pair_scalars(rng, opt, train, N, M, S, per_point):
         if per_point:
             jit = (np.clip(0.04 * rng.randn(2, N, 3), -0.12, 0.12), np.clip(0.01 * rng.randn(2, N, S), -0.05, 0.05),
                    np.clip(0.04 * rng.randn(2, M, 3), -0.12, 0.12))
-        scale = rng.uniform(low=0.9, high=1.1)
+        scale = rng.uniform(low=scale_range[0], high=scale_range[1])
         shift = rng.uniform(-1, 1, (1, 3))
         p[0:9] = angles2rotation_matrix(angles_2d).ravel()
         p[9:18] = angles2rotation_matrix(angles_3d).ravel()
@@ -121,9 +121,10 @@ def draw_pair_scalars(rng, opt, train, N, M, S, per_point):
     return p, jit
 
 
-def _step_rng(seed, step):
+def _step_rng(seed, step, stream=0):
+    """The host RandomState of (seed, step); a nonzero `stream` gives an independent one for other per-batch draws."""
     w = [(seed >> s) & 0xffffffff for s in (0, 32)] + [(step >> s) & 0xffffffff for s in (0, 32)]
-    return np.random.RandomState(np.array(w, dtype=np.uint32))
+    return np.random.RandomState(np.array(w + ([stream] if stream else []), dtype=np.uint32))
 
 
 # ----------------------------------------------------------------------------------------------- the builders
@@ -131,7 +132,8 @@ class _PairBuilder:
     """What the detector's and the descriptor's pair builders share.  A batch of B pairs is 2B clouds, cloud 2b + side
     (side 0 = src / anchor, 1 = dst / positive) a subsample of one scan: subsets, FPS candidates and nodes are built per
     cloud, whichever scans a pair's two clouds come from.  A subclass names the scan of every cloud (`_clouds`), draws
-    one pair's scalars (`_draw`) and runs its augment kernel (`_augment`).
+    one pair's scalars (`_draw`) and runs its augment kernel (`_augment`); it may reorder parity mode's draws of one
+    item (`_draw_item`) and scale the FPS candidates' z (`_z_scale`).
 
     rng="device": per-point randomness (subsets, jitter, FPS start) is Philox keyed by (seed, step, cloud, point,
     purpose); per-pair scalars come from a numpy RandomState seeded by (seed, step).  Host work is O(B) and a given
@@ -183,6 +185,17 @@ class _PairBuilder:
 
     def _augment(self, scans, offsets, scan_of_cloud, rows, nodes, params, step, jit):
         raise NotImplementedError
+
+    def _draw_item(self, rng, n_valid):
+        """Parity mode: every draw of one item, in its loader's order -> ([(rows, cand, start) of side 0, of side 1],
+        `_draw(rng, True)`'s result).  n_valid: the drawable rows of the item's two clouds.  By default each side's
+        get_instance_unaugmented_np (rows, FPS candidates, FPS start), then the pair's augmentation."""
+        sides = [draw_subsample(rng, n, self.N, self.divisor) for n in n_valid]
+        return sides, self._draw(rng, True)
+
+    def _z_scale(self, params):
+        """(2B,) f32 factors of the FPS candidates' z, from the host params (B or 2B blocks), or None (no scaling)."""
+        return None
 
     def _build(self, scans, offsets, step, *items):
         offsets = np.asarray(offsets, dtype=np.int64)
@@ -236,18 +249,22 @@ class _PairBuilder:
                 start_h = np.empty((2 * B,), np.int32)
                 drawn = []
                 for b in range(B):                     # the reference's __getitem__, item by item
-                    for c in (2 * b, 2 * b + 1):
-                        n_valid = int(lengths[c]) if drawable is None else len(drawable[c])
-                        choice, cand_h[c], start_h[c] = draw_subsample(np.random, n_valid, N, self.divisor)
+                    pair = (2 * b, 2 * b + 1)
+                    sides, d = self._draw_item(np.random, [int(lengths[c]) if drawable is None else len(drawable[c])
+                                                           for c in pair])
+                    for c, (choice, cand_h[c], start_h[c]) in zip(pair, sides):
                         rows_h[c] = choice if drawable is None else drawable[c][choice]
-                    drawn.append(self._draw(np.random, True))
+                    drawn.append(d)
                 rows, cand, start = up(rows_h), up(cand_h), up(start_h)
                 if drawn[0][1] is not None:            # per cloud (2, n, k) -> (2B, n, k); per pair (n, k) -> (B, n, k)
                     jit = tuple(up(np.stack([d[1][k] for d in drawn]).reshape((-1,) + drawn[0][1][k].shape[-2:]))
                                 for k in range(3))
-            params = np.stack([d[0] for d in drawn])
-            params = up(params.reshape(-1, params.shape[-1]))
-            pts = ops.cloud_gather_candidates(scans, offsets_d, scan_of_cloud, rows, cand)
+            params_h = np.stack([d[0] for d in drawn])
+            params_h = params_h.reshape(-1, params_h.shape[-1])
+            params = up(params_h)
+            zs = self._z_scale(params_h)
+            pts = ops.cloud_gather_candidates(scans, offsets_d, scan_of_cloud, rows, cand,
+                                              None if zs is None else up(zs))
             _, nodes = ops.fps(pts, start, M, want_nodes=True)
             out = self._augment(scans, offsets_d, scan_of_cloud, rows, nodes, params, step, jit)
         self.last = {"rows": rows, "cand": cand, "start": start, "candidates": pts, "params": params}
@@ -352,15 +369,16 @@ def synthetic_scan(seed, Ns, C=8):
 
 class _ScanSource:
     """What every device-built pair source shares, whatever its tree: a list of `.npy` scans (`paths[i]` is the scan of
-    item i) loaded once into pinned host memory, or onto the device with resident="device"; shuffled epochs; and the
+    item i, unless a subclass indexes them itself) loaded once into pinned host memory, or onto the device with resident="device"; shuffled epochs; and the
     hand-over.  Iteration builds batch i+1 on a stream of its own while the caller runs step i, and hands each batch over
     with `model.prefetch_input(..., after=event)` + `set_input()`: the model's stream waits on the build's event, the
     host never synchronises.  Every batch is a fresh set of tensors, so a batch still in use is never overwritten.  A
     subclass turns the item indices of one batch into the model's inputs (`_build`, called with the build stream
     current)."""
 
-    def __init__(self, paths, mode, opt, builder, device, seed, resident, rng, batch_size, drop_last):
+    def __init__(self, paths, mode, opt, builder, device, seed, resident, rng, batch_size, drop_last, n_items=None):
         self.opt, self.mode = opt, mode
+        self.n_items = len(paths) if n_items is None else int(n_items)   # items 0..n_items-1; by default scan i
         self.device = torch.device(device if device is not None else "cuda")
         self.batch_size = int(batch_size or opt.batch_size)
         self.drop_last = drop_last
@@ -377,7 +395,7 @@ class _ScanSource:
         self.last = None                        # what the batch last yielded was built from, for inspection
 
     def __len__(self):
-        n = len(self.offsets) - 1
+        n = self.n_items
         return n // self.batch_size if self.drop_last else -(-n // self.batch_size)
 
     def _build(self, items):
@@ -394,7 +412,7 @@ class _ScanSource:
 
     def batches(self):
         """One shuffled epoch of (input tensors, ready event); batch i+1 is enqueued before batch i is yielded."""
-        perm = self.order_rng.permutation(len(self.offsets) - 1)
+        perm = self.order_rng.permutation(self.n_items)
         chunks = [perm[i:i + self.batch_size] for i in range(0, len(perm), self.batch_size)]
         if self.drop_last and chunks and len(chunks[-1]) < self.batch_size:
             chunks.pop()

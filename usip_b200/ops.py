@@ -139,6 +139,7 @@ def fps(pts, start, k, want_nodes=True):
 
 # ----------------------------------------------------------------------------- training pairs (csrc/pairgen.cu)
 PAIR_TRAIN, PAIR_ROT_HORIZONTAL, PAIR_ROT_3D, PAIR_ROT_PERTURBATION, PAIR_TRANSLATION = 1, 2, 4, 8, 16
+PAIR_ENU_TO_CAM, PAIR_HEIGHT_SCALE = 32, 64      # Oxford: camera frame first; detector height scale = params[:, 44]
 PAIR_PARAM_STRIDE = 48                           # detector: doubles per pair
 DESC_PARAM_STRIDE = 32                           # descriptor: doubles per cloud
 
@@ -179,16 +180,41 @@ def cloud_subsample(scans, offsets, scan_of_cloud, max_rows, N, n_cand, radius=N
     return rows, cand, start, valid
 
 
-def cloud_gather_candidates(scans, offsets, scan_of_cloud, rows, cand):
-    """FPS input: (2B, n_cand, 3) f32 xyz of rows[c, cand[c, j]] of scan scan_of_cloud[c]."""
+def cloud_gather_candidates(scans, offsets, scan_of_cloud, rows, cand, z_scale=None):
+    """FPS input: (2B, n_cand, 3) f32 xyz of rows[c, cand[c, j]] of scan scan_of_cloud[c].  z_scale (2B,) f32 or
+    None: z becomes fl32(z * z_scale[c]) (the Oxford detector's height scaling)."""
     _req_scans(scans, offsets, scan_of_cloud); _req(rows, i32, "rows"); _req(cand, i32, "cand")
     B, N, n_cand = scan_of_cloud.shape[0] // 2, rows.shape[1], cand.shape[1]
     pts = torch.empty((2 * B, n_cand, 3), dtype=f32, device=scans.device)
+    lib = _lib.load()
     with torch.cuda.device(scans.device):
-        check(_lib.load().usip_cloud_gather_candidates(_p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud),
-                                                       _p(rows), _p(cand), _p(pts), B, N, n_cand, _stream()),
-              "usip_cloud_gather_candidates")
+        if z_scale is None:
+            check(lib.usip_cloud_gather_candidates(_p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows),
+                                                   _p(cand), _p(pts), B, N, n_cand, _stream()),
+                  "usip_cloud_gather_candidates")
+        else:
+            _req(z_scale, f32, "z_scale")
+            if tuple(z_scale.shape) != (2 * B,):
+                raise ValueError("z_scale must be (%d,), one factor per cloud; got %s" % (2 * B, tuple(z_scale.shape)))
+            check(lib.usip_cloud_gather_candidates_zscaled(_p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud),
+                                                           _p(rows), _p(cand), _p(z_scale), _p(pts), B, N, n_cand,
+                                                           _stream()), "usip_cloud_gather_candidates_zscaled")
     return pts
+
+
+def scale_channel_(t, k, factor):
+    """In place: t[:, k, :] *= factor for t (B, C, L) f32 CUDA, in fp32 as torch multiplies a float32 tensor by a
+    Python float.  Returns t."""
+    _req(t, f32, "t")
+    if t.dim() != 3 or not 0 <= int(k) < t.shape[1]:
+        raise ValueError("t must be (B, C, L) with 0 <= k < C")
+    B, C, L = t.shape
+    if t.numel() == 0:
+        return t
+    with torch.cuda.device(t.device):
+        check(_lib.load().usip_scale_channel_f32(_p(t), B, C, L, int(k), float(factor), _stream()),
+              "usip_scale_channel_f32")
+    return t
 
 
 def pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, S, flags, seed=0, step=0, jit_pc=None, jit_sn=None,
