@@ -163,6 +163,33 @@ int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, co
                            int n_pairs, int N, int M, float* anc_pc, float* anc_sn, float* anc_node, float* pos_pc,
                            float* pos_sn, float* pos_node, void* stream);
 
+/* Test-set clouds (evaluation/kitti_test_loader.py:106-139, oxford_test_loader.py:63-96; the noise of
+ * evaluation/save_keypoints.py:275).  n_clouds clouds, cloud c reading scan scan_of_cloud[c]: rows (n_clouds, N) i32
+ * and FPS nodes (n_clouds, 3, M) f32 (usip_cloud_subsample / usip_cloud_gather_candidates / usip_fps_f32) ->
+ * pc (n_clouds, 3, N), sn (n_clouds, S, N) = scan columns 3:3+S, node (n_clouds, 3, M).  flags: 0 or
+ * USIP_PAIR_ENU_TO_CAM (Oxford: pc, sn columns 0:3 and nodes to the camera frame, S >= 3).  With noise_sigma != 0, pc
+ * then becomes fl32(pc + fl32(n * fl32(noise_sigma))) with n uploaded in noise (n_clouds, 3, N) f32 (torch.randn on the
+ * host), or, with noise NULL, a Philox N(0, 1) keyed by (seed, step, cloud, point). */
+int usip_test_cloud_gather(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                           const int32_t* rows, const float* nodes, const float* noise, float noise_sigma,
+                           uint64_t seed, uint64_t step, int flags, int S, int n_clouds, int N, int M, float* pc,
+                           float* sn, float* node, void* stream);
+
+/* Keypoint repeatability       evaluation/matlab/eval_repeatability/eval_rep.m:142-146, for every K of a sweep at once.
+ * keypoints (n_scans, 3, M) f32, order (n_scans, M) i32 (the selection order of every scan's keypoints), count
+ * (n_scans,) i32 (how many of them are selectable).  pairs (P, 2) i32: the anchor and positive scan.  frames (P, 3, 3, 4)
+ * f64 row-major: the anchor's frame map F_a, the positive's F_p and the ground truth T_gt.  ks: nK ascending positive
+ * K values (host memory, nK <= USIP_REP_MAX_K).  For pair p and K = ks[k], with n_a = min(K, count[anc]) and
+ * n_p = min(K, count[pos]):  a_i = F_a * kp[anc][:, order[anc][i]] (i < n_a),  q_j = T_gt * (F_p * kp[pos][:,
+ * order[pos][j]]) (j < n_p), each matrix-vector product ((m0 x + m1 y) + m2 z) + m3 in fp64 without contraction;
+ * inliers[p, k] = #{i : sqrt(min_j ((dx^2 + dy^2) + dz^2)) < radius} and n_anc[p, k] = n_a.  One CTA per pair;
+ * min(M, ks[nK-1]) must not exceed USIP_REP_MAX_KEYPOINTS, radius must be > 0. */
+#define USIP_REP_MAX_K 32
+#define USIP_REP_MAX_KEYPOINTS 4096
+int usip_repeatability_f64(const float* keypoints, const int32_t* order, const int32_t* count, int n_scans, int M,
+                           const int32_t* pairs, const double* frames, int P, const int32_t* ks, int nK, double radius,
+                           int32_t* inliers, int32_t* n_anc, void* stream);
+
 /* Radius non-maximum suppression of the detected keypoints    evaluation/save_keypoints.py:180-216 (nms)
  * keypoints (B,3,M) f32, sigmas (B,M) f32 -> out_idx (B,M) i32: original indices of the kept keypoints in the order the
  * reference emits them (ascending sigma, ties by index), padded with -1; out_count (B,) i32.  radius < 0.01: pass-through

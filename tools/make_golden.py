@@ -562,6 +562,99 @@ def golden_oxford_descpairs(ref):
     print("oxford_descpairs.npz", os.path.getsize(os.path.join(OUT, "oxford_descpairs.npz")) // 1024, "KB")
 
 
+# evaluation/kitti_test_loader.py KittiTestLoader and evaluation/oxford_test_loader.py OxfordTestLoader, batched by
+# default_collate as save_keypoints.py's DataLoader does, plus save_keypoints.py:275's noise per batch, on synthetic
+# test trees (usip_b200.evaluation.*.write_synthetic_*_test).  The index draws (rows, FPS candidates, FPS start) are
+# logged from np.random as the loaders make them.  Five scans in batches of two: the last batch is odd.
+TEST_COUNTS, TEST_PAIRS = [3, 2], [[(0, 1), (2, 1), (0, 2)], [(1, 0)]]
+TEST_OX_NUMBERS, TEST_OX_PAIRS = [0, 1, 2, 3, 4], [(0, 1), (3, 2), (4, 4)]
+TEST_ROWS, TEST_SEED, TEST_N, TEST_M, TEST_B = 1300, 7500, 512, 32, 2
+TEST_CASES = {"plain": (61, 0.0), "noise": (62, 0.05)}      # name: (np / torch seed, noise sigma)
+
+
+def _golden_test_clouds(ref, module, make_loader, write_tree, out_name):
+    import importlib
+    import tempfile
+    from torch.utils.data.dataloader import default_collate
+    if ref_shim.build_ref_root() not in sys.path:
+        sys.path.insert(0, ref_shim.build_ref_root())
+    try:
+        import PIL.Image  # noqa: F401               util/vis_tools.py imports it; only its plots use it
+    except ImportError:
+        import types
+        sys.modules["PIL"] = types.ModuleType("PIL")
+        sys.modules["PIL"].__dict__.update(Image=None, ImageMath=None)
+    tl = importlib.import_module("evaluation." + module)
+    out = {"tree/rows": np.int64(TEST_ROWS), "tree/seed": np.int64(TEST_SEED), "N": np.int64(TEST_N),
+           "M": np.int64(TEST_M), "batch_size": np.int64(TEST_B)}
+    draws = []
+    np_choice, np_randint = np.random.choice, np.random.randint
+
+    def choice(a, size=None, replace=True, p=None):
+        r = np_choice(a, size, replace, p)
+        draws.append(np.asarray(r))
+        return r
+
+    def randint(low, high=None, size=None, dtype=int):
+        r = np_randint(low, high, size, dtype)
+        draws.append(np.asarray(r))
+        return r
+    with tempfile.TemporaryDirectory() as root:
+        write_tree(root)
+        opt = ref_shim.make_opt(input_pc_num=TEST_N, node_num=TEST_M, surface_normal_len=4)
+        loader = make_loader(tl, root, opt)
+        np.random.choice, np.random.randint = choice, randint
+        try:
+            for name, (seed, sigma) in TEST_CASES.items():
+                np.random.seed(seed)
+                torch.manual_seed(seed)
+                del draws[:]
+                res = {"pc": [], "sn": [], "node": []}
+                for b0 in range(0, len(loader), TEST_B):
+                    batch = default_collate([loader[i] for i in range(b0, min(b0 + TEST_B, len(loader)))])
+                    pc = batch[0]
+                    if sigma:
+                        pc = pc + torch.randn(pc.size()) * sigma
+                    for k, v in zip(("pc", "sn", "node"), (pc, batch[1], batch[2])):
+                        res[k].append(v.numpy())
+                out[name + "/case"] = np.array([seed], dtype=np.int64)
+                out[name + "/noise_sigma"] = np.float64(sigma)
+                for k, v in res.items():
+                    out[name + "/" + k] = np.concatenate(v)
+                out[name + "/rows"] = np.stack(draws[0::3]).astype(np.int32)
+                out[name + "/cand"] = np.stack(draws[1::3]).astype(np.int32)
+                out[name + "/start"] = np.array(draws[2::3], dtype=np.int32)
+                print(out_name, name, {k: out[name + "/" + k].shape for k in ("pc", "sn", "node", "rows", "cand")})
+        finally:
+            np.random.choice, np.random.randint = np_choice, np_randint
+    np.savez_compressed(os.path.join(OUT, out_name), **out)
+    print(out_name, os.path.getsize(os.path.join(OUT, out_name)) // 1024, "KB")
+
+
+def golden_kitti_test(ref):
+    from usip_b200.evaluation.kitti_test_loader import write_synthetic_kitti_test
+    _golden_test_clouds(
+        ref, "kitti_test_loader",
+        lambda tl, root, opt: tl.KittiTestLoader(os.path.join(root, "txt"), os.path.join(root, "numpy"), opt),
+        lambda root: write_synthetic_kitti_test(os.path.join(root, "txt"), os.path.join(root, "numpy"),
+                                                os.path.join(root, "calib"), TEST_COUNTS, TEST_ROWS, TEST_PAIRS,
+                                                seed=TEST_SEED),
+        "kitti_test_clouds.npz")
+
+
+def golden_oxford_test(ref):
+    from usip_b200.evaluation.oxford_test_loader import write_synthetic_oxford_test
+    def make_loader(tl, root, opt):
+        loader = tl.OxfordTestLoader(root, opt)
+        loader.dataset = list(TEST_OX_NUMBERS)           # the synthetic tree has 5 of the 828 test scans
+        return loader
+    _golden_test_clouds(
+        ref, "oxford_test_loader", make_loader,
+        lambda root: write_synthetic_oxford_test(root, TEST_OX_NUMBERS, TEST_ROWS, TEST_OX_PAIRS,
+                                                 os.path.join(root, "groundtruths.txt"), seed=TEST_SEED),
+        "oxford_test_clouds.npz")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)

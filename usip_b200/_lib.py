@@ -76,6 +76,10 @@ SIGNATURES = {
     "usip_desc_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                        ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
                                + [c_ptr] * 6 + [c_ptr]),
+    "usip_test_cloud_gather": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_f32, ctypes.c_uint64,
+                                       ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int, c_ptr, c_ptr, c_ptr, c_ptr]),
+    "usip_repeatability_f64": (c_int, [c_ptr, c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_ptr, c_int,
+                                       ctypes.c_double, c_ptr, c_ptr, c_ptr]),
     "usip_nms_f32":(c_int, [c_ptr, c_ptr, ctypes.c_float, c_ptr, c_ptr, c_int, c_int, c_ptr]),
     "usip_l2norm_bwd": (c_int, [c_ptr, c_ptr, c_int, c_ptr, c_int, c_int, c_int, c_int, c_ptr]),
     "usip_desc_triplet_bwd": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, ctypes.c_float, ctypes.c_float,

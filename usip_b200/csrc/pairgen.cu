@@ -24,7 +24,7 @@ constexpr int PG_PARAM_STRIDE = 48;                // doubles per pair, see usip
 constexpr int PG_DESC_PARAM_STRIDE = 32;           // doubles per cloud, see usip_desc_pair_augment in the header
 
 enum { PURPOSE_ROWS = 0, PURPOSE_CAND = 1, PURPOSE_START = 2, PURPOSE_JIT_PC = 3, PURPOSE_JIT_SN = 4,
-       PURPOSE_JIT_NODE = 5 };
+       PURPOSE_JIT_NODE = 5, PURPOSE_NOISE = 6 };
 
 // ---------------------------------------------------------------------------------------------- Philox4x32-10
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
@@ -559,6 +559,53 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
   }
 }
 
+// Test-set clouds (KittiTestLoader / OxfordTestLoader.__getitem__, then save_keypoints.py:275's noise): no
+// augmentation, no dst.  The rows and nodes as they are, moved to the camera frame under USIP_PAIR_ENU_TO_CAM (after
+// FPS, as the Oxford loader does); then `anc_pc + torch.randn(size) * sigma`, a float32 tensor times a Python float.
+__global__ void __launch_bounds__(PG_AUG_THREADS)
+test_cloud_gather_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
+                         const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
+                         const float* __restrict__ nodes, const float* __restrict__ noise, float sigma, uint64_t seed,
+                         uint64_t step, int flags, int S, int N, int M, float* __restrict__ pc, float* __restrict__ sn_out,
+                         float* __restrict__ node_out) {
+  const int c = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) {
+    const float* p = scans + (offsets[scan_of_cloud[c]] + rows[(int64_t)c * N + i]) * C;
+    float x = p[0], y = p[1], z = p[2];
+    float sn[PG_MAX_S];
+#pragma unroll
+    for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[3 + k] : 0.f;
+    pg_enu_to_cam(flags, 1.0, y, z, sn, S);
+    float* o = pc + (int64_t)c * 3 * N;
+    if (sigma != 0.f) {
+      float n[3];
+      if (noise) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) n[k] = noise[((int64_t)c * 3 + k) * N + i];
+      } else {
+        const uint4 u = pg_random(seed, step, c, i, PURPOSE_NOISE, 0);
+        double z0, z1, z2, z3;
+        pg_normal2(u.x, u.y, z0, z1); pg_normal2(u.z, u.w, z2, z3);
+        n[0] = (float)z0; n[1] = (float)z1; n[2] = (float)z2;
+      }
+      x = __fadd_rn(x, __fmul_rn(n[0], sigma));
+      y = __fadd_rn(y, __fmul_rn(n[1], sigma));
+      z = __fadd_rn(z, __fmul_rn(n[2], sigma));
+    }
+    o[i] = x; o[N + i] = y; o[2 * N + i] = z;
+#pragma unroll
+    for (int k = 0; k < PG_MAX_S; ++k)
+      if (k < S) sn_out[((int64_t)c * S + k) * N + i] = sn[k];
+  }
+  if (i < M) {
+    const float* nd = nodes + (int64_t)c * 3 * M;
+    float x = nd[i], y = nd[M + i], z = nd[2 * M + i];
+    pg_enu_to_cam(flags, 1.0, y, z, nullptr, 0);
+    float* o = node_out + (int64_t)c * 3 * M;
+    o[i] = x; o[M + i] = y; o[2 * M + i] = z;
+  }
+}
+
 // t[b, k, :] *= f in fp32 (torch's `t[:, k, :] *= f` with f a Python float: fl32(v * fl32(f)))
 __global__ void scale_channel_kernel(float* __restrict__ t, int C, int L, int k, float f) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -632,6 +679,22 @@ extern "C" int usip_scale_channel_f32(float* t, int B, int C, int L, int k, floa
   dim3 grid(cdiv(L, 256), B);
   scale_channel_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(t, C, L, k, factor);
   return check_launch("scale_channel_kernel");
+}
+
+extern "C" int usip_test_cloud_gather(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                                      const int32_t* rows, const float* nodes, const float* noise, float noise_sigma,
+                                      uint64_t seed, uint64_t step, int flags, int S, int n_clouds, int N, int M,
+                                      float* pc, float* sn, float* node, void* stream) {
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes, "test_cloud_gather: null input");
+  USIP_REQUIRE(pc && sn && node, "test_cloud_gather: null output");
+  USIP_REQUIRE(S >= 1 && S <= PG_MAX_S && 3 + S <= C, "test_cloud_gather: bad surface-normal length");
+  USIP_REQUIRE((flags & ~USIP_PAIR_ENU_TO_CAM) == 0, "test_cloud_gather: only USIP_PAIR_ENU_TO_CAM applies");
+  USIP_REQUIRE(!(flags & USIP_PAIR_ENU_TO_CAM) || S >= 3, "test_cloud_gather: the camera frame needs S >= 3");
+  USIP_REQUIRE(n_clouds > 0 && n_clouds <= 65535 && N > 0 && M > 0, "test_cloud_gather: bad sizes");
+  dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), n_clouds);
+  test_cloud_gather_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
+      scans, C, offsets, scan_of_cloud, rows, nodes, noise, noise_sigma, seed, step, flags, S, N, M, pc, sn, node);
+  return check_launch("test_cloud_gather_kernel");
 }
 
 extern "C" int usip_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,

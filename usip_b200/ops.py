@@ -274,6 +274,52 @@ def desc_pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, S, fla
     return out
 
 
+def test_cloud_gather(scans, offsets, scan_of_cloud, rows, nodes, S, flags=0, noise_sigma=0.0, noise=None, seed=0,
+                      step=0):
+    """Test-set clouds (no augmentation, no pair) -> (pc (B,3,N), sn (B,S,N), node (B,3,M)) f32, B = len(scan_of_cloud).
+    flags: 0 or PAIR_ENU_TO_CAM.  noise_sigma != 0 adds fl32(n * sigma) to pc, n = noise (B,3,N) f32 or, when None,
+    Philox N(0, 1) drawn from (seed, step)."""
+    _req(scans, f32, "scans"); _req(offsets, torch.int64, "offsets"); _req(scan_of_cloud, i32, "scan_of_cloud")
+    _req(rows, i32, "rows"); _req(nodes, f32, "nodes")
+    B, N, M, dev = scan_of_cloud.shape[0], rows.shape[1], nodes.shape[2], scans.device
+    if scans.dim() != 2 or rows.shape[0] != B or tuple(nodes.shape[:2]) != (B, 3):
+        raise ValueError("scans [T, C], rows (B, N), nodes (B, 3, M) with B = len(scan_of_cloud)")
+    if noise is not None:
+        _req(noise, f32, "noise")
+        if tuple(noise.shape) != (B, 3, N):
+            raise ValueError("noise must be (%d, 3, %d); got %s" % (B, N, tuple(noise.shape)))
+    e = lambda *s: torch.empty(s, dtype=f32, device=dev)
+    out = (e(B, 3, N), e(B, int(S), N), e(B, 3, M))
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_test_cloud_gather(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows), _p(nodes), _p(noise),
+            float(noise_sigma), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), int(flags), int(S), B, N, M,
+            *[_p(t) for t in out], _stream()), "usip_test_cloud_gather")
+    return out
+
+
+def repeatability(keypoints, order, count, pairs, frames, ks, radius):
+    """eval_rep.m's inlier counts for every K at once (include/usip_b200.h usip_repeatability_f64).  keypoints
+    (S,3,M) f32, order (S,M) i32, count (S,) i32, pairs (P,2) i32, frames (P,3,3,4) f64 (F_a, F_p, T_gt), all CUDA;
+    ks ascending ints (host) -> (inliers (P,nK) i32, n_anc (P,nK) i32)."""
+    _req(keypoints, f32, "keypoints"); _req(order, i32, "order"); _req(count, i32, "count")
+    _req(pairs, i32, "pairs"); _req(frames, torch.float64, "frames")
+    S, _, M = keypoints.shape
+    P = pairs.shape[0]
+    if tuple(order.shape) != (S, M) or tuple(count.shape) != (S,):
+        raise ValueError("order must be (%d, %d) and count (%d,)" % (S, M, S))
+    if pairs.dim() != 2 or pairs.shape[1] != 2 or tuple(frames.shape) != (P, 3, 3, 4):
+        raise ValueError("pairs must be (P, 2) and frames (P, 3, 3, 4)")
+    ks_h = (ctypes.c_int32 * len(ks))(*[int(k) for k in ks])
+    inl = torch.empty((P, len(ks)), dtype=i32, device=keypoints.device)
+    n_anc = torch.empty((P, len(ks)), dtype=i32, device=keypoints.device)
+    with torch.cuda.device(keypoints.device):
+        check(_lib.load().usip_repeatability_f64(
+            _p(keypoints), _p(order), _p(count), S, M, _p(pairs), _p(frames), P, ks_h, len(ks), float(radius),
+            _p(inl), _p(n_anc), _stream()), "usip_repeatability_f64")
+    return inl, n_anc
+
+
 def nms(keypoints, sigmas, radius):
     """keypoints (B,3,M) f32, sigmas (B,M) f32 -> (idx (B,M) i32 kept indices in emission order, -1 padded; count (B,) i32)."""
     _req(keypoints, f32, "keypoints"); _req(sigmas, f32, "sigmas")
