@@ -190,6 +190,66 @@ int usip_repeatability_f64(const float* keypoints, const int32_t* order, const i
                            const int32_t* pairs, const double* frames, int P, const int32_t* ks, int nK, double radius,
                            int32_t* inliers, int32_t* n_anc, void* stream);
 
+/* Outdoor registration    evaluation/matlab/eval_outdoor/{kitti/evaluate_kitti.m, oxford/evaluate_oxford.m}: descriptor
+ * matching, then RANSAC (external/ransacfitRt.m, ransac.m, estimateRigidTransform.m), for every pair, every K of a
+ * keypoint-count sweep and every trial budget of a maxTrials sweep.  Both kernels run one CTA per (pair, K) and refuse
+ * more than USIP_REG_MAX_KEYPOINTS rows per scan (their shared memory).
+ *
+ * usip_desc_match_f64: desc (n_scans, L, D) f32, each scan's rows in selection order; count (n_scans,) i32; pairs
+ * (P, 2) i32 (anchor scan, positive scan); ks: nK ascending positive K values (host memory, nK <= USIP_REP_MAX_K).  For
+ * pair p and K = ks[kk] the anchor set is rows 0..n_a-1 of the anchor scan, n_a = min(K, count, L), and likewise the
+ * positive set.  d^2(i, j) = sum_c (a_c - b_c)^2 in fp64 with c ascending and no contraction; candidates are ordered
+ * by (d^2, index), so the lowest index wins a tie, and a NaN d^2 (a non-finite descriptor value) orders as +inf: every
+ * row gets its min(k, n) neighbours whatever the values.
+ *   k == 1 (KITTI): one-way 1-NN; match i = (i, nearest positive) for i < n_a, in anchor order (none if n_pos = 0).
+ *   k in 2..8 (Oxford): the k nearest positives of every anchor united with the k nearest anchors of every positive
+ *   (all rows when a set has fewer than k), unique rows sorted by anchor, then positive: MATLAB's union(.., 'rows').
+ * -> matches (P, nK, cap, 2) i32 (anchor row, positive row), cap = L for k == 1 and 2*k*L otherwise, and n_matches
+ * (P, nK) i32.  D must not exceed USIP_REG_MAX_DIM.
+ *
+ * usip_ransac_rt_f64: xyz (n_scans, L, 3) f32 in the rows' order of desc; count, pairs as above; frames (P, 3, 3, 4)
+ * f64 (F_a, F_p, T_gt as usip_repeatability_f64; T_gt is not read); matches / n_matches of usip_desc_match_f64 (cap
+ * as there); trials: nT ascending trial budgets (host memory, 1 <= nT <= USIP_REG_MAX_SWEEP, 1 <= trials[i] <=
+ * USIP_REG_MAX_TRIALS); threshold > 0.  x1 = F_a * anchor row, x2 = F_p * positive row (((m0 x + m1 y) + m2 z) + m3),
+ * and the model is x1 = R x2 + t.
+ *   Trial j (0-based) reads three uniforms u in [0, 1): row j of uniforms ((trials[nT-1] + 1, 3) f64) when given, else
+ *   Philox4x32-10 with counter (j, 0, 0x52414e53, 0) and key (seed lo, seed hi), u_i = word_i * 2^-32 (i = 0, 1, 2):
+ *   every pair and K sees the same stream, as ransac.m's rng(0) does.  usip_ransac_uniforms writes them.
+ *   Sample of n = npts matches: i0 = min(floor(u0 n), n-1); i1 = min(floor(u1 (n-1)), n-2), then i1 += 1 if i1 >= i0;
+ *   i2 = min(floor(u2 (n-2)), n-3), then i2 += 1 if i2 >= min(i0, i1), then i2 += 1 if i2 >= max(i0, i1); products
+ *   in fp64.
+ *   Fit (estimateRigidTransform.m): centroids ((0 + p_0) + p_1) + ... then / n; B = sum of A_i^T A_i over the points in
+ *   order, A_i = [0, (y-x)^T; x-y, [y+x]_x] of the centred pair, entry (r, c) ((A0r A0c + A1r A1c) + A2r A2c) + A3r A3c;
+ *   cyclic Jacobi on B, pairs (0,1) (0,2) (0,3) (1,2) (1,3) (2,3), 8 sweeps, a rotation skipped when its off-diagonal
+ *   entry is exactly 0 (theta = (a_qq - a_pp) / (2 a_pq), t = sign(theta) / (|theta| + sqrt(theta^2 + 1)), sign(0) =
+ *   1, c = 1 / sqrt(t^2 + 1), s = t c); the eigenvector of the smallest diagonal entry (lowest index on a tie) goes
+ *   to quat2rot.m unnormalised; t = xbar - R ybar.  Inlier: sqrt((dx^2 + dy^2) + dz^2) < threshold, strictly.
+ *   Stop (ransac.m): on ninliers >= bestscore the trial becomes the best and N = max(log(1 - 0.99) / log(clamp(1 -
+ *   (f f) f, eps, 1 - eps)), 10), f = ninliers / npts; then trialcount += 1; the loop ends when trialcount > maxTrials
+ *   or N <= trialcount.  One stream serves the whole sweep: each budget's result is the loop state where that loop
+ *   ends.  Trials run 256 at a time and one thread replays the update in trial order, so the result is the sequential
+ *   loop's.  `log` is CUDA's, within 1 ulp of a correctly rounded one, so a stop can differ from another libm's only
+ *   when N lies within an ulp of an integer; every other step is correctly rounded.
+ *   Finish (ransacfitRt.m): the best trial's inliers are refitted as above (status 0), unless fewer than 3 (status 2,
+ *   Rt zero).  npts < 3: status 1, no model; npts == 3: fitted directly, trialcount 0, n_inliers 3.  A match index
+ *   outside its scan's rows gives status 3.
+ * -> Rt (P, nK, nT, 3, 4) f64; n_inliers (the best trial's count), trialcount, best_trial (-1 without trials) and
+ * status, each (P, nK, nT) i32. */
+#define USIP_REG_MAX_KEYPOINTS 1024
+#define USIP_REG_MAX_DIM 512
+#define USIP_REG_MAX_MATCH_K 8
+#define USIP_REG_MAX_SWEEP 16
+#define USIP_REG_MAX_TRIALS 100000
+int usip_desc_match_f64(const float* desc, const int32_t* count, int n_scans, int L, int D, const int32_t* pairs,
+                        int P, const int32_t* ks, int nK, int k, int32_t* matches, int32_t* n_matches, void* stream);
+int usip_ransac_rt_f64(const float* xyz, const int32_t* count, int n_scans, int L, const int32_t* pairs,
+                       const double* frames, int P, int nK, const int32_t* matches, const int32_t* n_matches, int cap,
+                       const int32_t* trials, int nT, double threshold, uint64_t seed, const double* uniforms,
+                       double* Rt, int32_t* n_inliers, int32_t* trialcount, int32_t* best_trial, int32_t* status,
+                       void* stream);
+/* the uniforms of trials 0..T-1 of usip_ransac_rt_f64's Philox stream -> out (T, 3) f64 */
+int usip_ransac_uniforms(uint64_t seed, int T, double* out, void* stream);
+
 /* Radius non-maximum suppression of the detected keypoints    evaluation/save_keypoints.py:180-216 (nms)
  * keypoints (B,3,M) f32, sigmas (B,M) f32 -> out_idx (B,M) i32: original indices of the kept keypoints in the order the
  * reference emits them (ascending sigma, ties by index), padded with -1; out_count (B,) i32.  radius < 0.01: pass-through

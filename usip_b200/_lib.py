@@ -80,6 +80,12 @@ SIGNATURES = {
                                        ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int, c_ptr, c_ptr, c_ptr, c_ptr]),
     "usip_repeatability_f64": (c_int, [c_ptr, c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_ptr, c_int,
                                        ctypes.c_double, c_ptr, c_ptr, c_ptr]),
+    "usip_desc_match_f64": (c_int, [c_ptr, c_ptr, c_int, c_int, c_int, c_ptr, c_int, c_ptr, c_int, c_int, c_ptr, c_ptr,
+                                    c_ptr]),
+    "usip_ransac_rt_f64": (c_int, [c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_ptr,
+                                   c_int, ctypes.c_double, ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
+                                   c_ptr]),
+    "usip_ransac_uniforms": (c_int, [ctypes.c_uint64, c_int, c_ptr, c_ptr]),
     "usip_nms_f32":(c_int, [c_ptr, c_ptr, ctypes.c_float, c_ptr, c_ptr, c_int, c_int, c_ptr]),
     "usip_l2norm_bwd": (c_int, [c_ptr, c_ptr, c_int, c_ptr, c_int, c_int, c_int, c_int, c_ptr]),
     "usip_desc_triplet_bwd": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, ctypes.c_float, ctypes.c_float,

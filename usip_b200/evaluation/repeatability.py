@@ -179,21 +179,28 @@ class Repeatability:
         self.frames = np.ascontiguousarray(frames, dtype=np.float64).reshape(-1, 3, 3, 4)
         if len(self.pairs) == 0 or len(self.pairs) != len(self.frames):
             raise ValueError("need one frame triple per ground-truth pair, and at least one pair")
-        self.keypoints = self.sigmas = self.order = self.count = None
+        self.keypoints = self.sigmas = self.order = self.count = self.descriptors = None
 
-    def detect(self, model, nms_radius=0.0, noise_sigma=0.0):
+    def detect(self, model, nms_radius=0.0, noise_sigma=0.0, descriptor=None):
         """Runs the detector over the whole test set and keeps every scan's keypoints (S, 3, M), sigmas (S, M) and
-        selection order / count on the device."""
+        selection order / count on the device.  With a ModelDescriptor `descriptor`, every batch is also described at
+        its keypoints, on the clouds the detector saw (noise included), and descriptors (S, D, M) are kept too."""
         src = self.source
         dev = src.device
         S, M = len(src), src.M
         kp = torch.empty((S, 3, M), dtype=torch.float32, device=dev)
         sg = torch.empty((S, M), dtype=torch.float32, device=dev)
+        desc = None
         for items, (pc, sn, node) in src.batches(noise_sigma):
             k, s = model.run_model(pc, sn, node)
             kp[items[0]:items[-1] + 1] = k
             sg[items[0]:items[-1] + 1] = s
-        self.keypoints, self.sigmas = kp, sg
+            if descriptor is not None:
+                d = descriptor.run_model(pc, sn, k)
+                if desc is None:
+                    desc = torch.empty((S, d.shape[1], M), dtype=torch.float32, device=dev)
+                desc[items[0]:items[-1] + 1] = d
+        self.keypoints, self.sigmas, self.descriptors = kp, sg, desc
         self.order, self.count = select_order(kp, sg, nms_radius)
 
     def score(self, keypoint_nums=DEFAULT_KEYPOINT_NUMS, inlier_radius=DEFAULT_INLIER_RADIUS):
@@ -275,13 +282,17 @@ def detector_opt(dataset, **over):
     return o
 
 
-def load_detector_checkpoint(model, path):
-    """torch.load + model_state_dict_convert_auto for one GPU (save_keypoints.py:168-177): a `module.` prefix is
-    stripped."""
+def load_checkpoint(net, path):
+    """torch.load + model_state_dict_convert_auto for one GPU (save_keypoints.py:168-177) into `net`: a `module.`
+    prefix is stripped."""
     sd = torch.load(path, map_location="cpu")
     if any(k.startswith("module.") for k in sd):
         sd = {k[7:]: v for k, v in sd.items()}
-    model.detector.load_state_dict(sd)
+    net.load_state_dict(sd)
+
+
+def load_detector_checkpoint(model, path):
+    load_checkpoint(model.detector, path)
     model.freeze_model()
 
 

@@ -320,6 +320,66 @@ def repeatability(keypoints, order, count, pairs, frames, ks, radius):
     return inl, n_anc
 
 
+def desc_match(desc, count, pairs, ks, k):
+    """Descriptor matches of evaluate_kitti.m (k == 1) / evaluate_oxford.m (k in 2..8) for every pair and K at once
+    (include/usip_b200.h usip_desc_match_f64).  desc (S,L,D) f32, count (S,) i32, pairs (P,2) i32, all CUDA; ks
+    ascending ints (host) -> (matches (P,nK,cap,2) i32, n_matches (P,nK) i32), cap = L for k == 1, 2*k*L otherwise."""
+    _req(desc, f32, "desc"); _req(count, i32, "count"); _req(pairs, i32, "pairs")
+    S, L, D = desc.shape
+    P = pairs.shape[0]
+    if tuple(count.shape) != (S,) or pairs.dim() != 2 or pairs.shape[1] != 2:
+        raise ValueError("count must be (%d,) and pairs (P, 2)" % S)
+    ks_h = (ctypes.c_int32 * len(ks))(*[int(v) for v in ks])
+    cap = (L if int(k) == 1 else 2 * int(k) * L) if 1 <= int(k) <= 8 else 1      # the C call refuses a bad k
+    matches = torch.empty((P, len(ks), cap, 2), dtype=i32, device=desc.device)
+    n = torch.empty((P, len(ks)), dtype=i32, device=desc.device)
+    with torch.cuda.device(desc.device):
+        check(_lib.load().usip_desc_match_f64(_p(desc), _p(count), S, L, D, _p(pairs), P, ks_h, len(ks), int(k),
+                                              _p(matches), _p(n), _stream()), "usip_desc_match_f64")
+    return matches, n
+
+
+def ransac_rt(xyz, count, pairs, frames, matches, n_matches, trials, threshold=1.0, seed=0, uniforms=None):
+    """ransacfitRt.m for every pair, K and trial budget at once (include/usip_b200.h usip_ransac_rt_f64).  xyz (S,L,3)
+    f32, count (S,) i32, pairs (P,2) i32, frames (P,3,3,4) f64, matches / n_matches from desc_match, all CUDA; trials
+    ascending ints (host); uniforms None (Philox from seed) or (trials[-1] + 1, 3) f64 CUDA -> dict of Rt
+    (P,nK,nT,3,4) f64 and n_inliers, trialcount, best_trial, status (P,nK,nT) i32."""
+    _req(xyz, f32, "xyz"); _req(count, i32, "count"); _req(pairs, i32, "pairs"); _req(frames, torch.float64, "frames")
+    _req(matches, i32, "matches"); _req(n_matches, i32, "n_matches")
+    S, L, _ = xyz.shape
+    P, nK, cap = matches.shape[0], matches.shape[1], matches.shape[2]
+    if tuple(xyz.shape) != (S, L, 3) or tuple(count.shape) != (S,) or tuple(pairs.shape) != (P, 2):
+        raise ValueError("xyz must be (S, L, 3), count (S,) and pairs (P, 2)")
+    if tuple(frames.shape) != (P, 3, 3, 4) or tuple(matches.shape) != (P, nK, cap, 2) or \
+            tuple(n_matches.shape) != (P, nK):
+        raise ValueError("frames must be (P, 3, 3, 4), matches (P, nK, cap, 2) and n_matches (P, nK)")
+    trials = [int(t) for t in trials]
+    if uniforms is not None:
+        _req(uniforms, torch.float64, "uniforms")
+        if not trials or tuple(uniforms.shape) != (max(trials) + 1, 3):
+            raise ValueError("uniforms must be (max(trials) + 1, 3)")
+    t_h = (ctypes.c_int32 * len(trials))(*trials)
+    nT, dev = len(trials), xyz.device
+    Rt = torch.empty((P, nK, nT, 3, 4), dtype=torch.float64, device=dev)
+    e = lambda: torch.empty((P, nK, nT), dtype=i32, device=dev)
+    out = {"Rt": Rt, "n_inliers": e(), "trialcount": e(), "best_trial": e(), "status": e()}
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_ransac_rt_f64(
+            _p(xyz), _p(count), S, L, _p(pairs), _p(frames), P, nK, _p(matches), _p(n_matches), cap, t_h, nT,
+            float(threshold), int(seed) & (2 ** 64 - 1), _p(uniforms), _p(Rt), _p(out["n_inliers"]),
+            _p(out["trialcount"]), _p(out["best_trial"]), _p(out["status"]), _stream()), "usip_ransac_rt_f64")
+    return out
+
+
+def ransac_uniforms(T, seed=0, device="cuda"):
+    """The uniforms ransac_rt draws for trials 0..T-1 from `seed` -> (T, 3) f64 CUDA."""
+    out = torch.empty((int(T), 3), dtype=torch.float64, device=device)
+    with torch.cuda.device(out.device):
+        check(_lib.load().usip_ransac_uniforms(int(seed) & (2 ** 64 - 1), int(T), _p(out), _stream()),
+              "usip_ransac_uniforms")
+    return out
+
+
 def nms(keypoints, sigmas, radius):
     """keypoints (B,3,M) f32, sigmas (B,M) f32 -> (idx (B,M) i32 kept indices in emission order, -1 padded; count (B,) i32)."""
     _req(keypoints, f32, "keypoints"); _req(sigmas, f32, "sigmas")
