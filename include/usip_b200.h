@@ -92,7 +92,11 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *     (The descriptor's reference raises below N rows; its callers reject such scans.)
  *   out_cand (2*n_pairs, n_cand) i32: a uniform subset of n_cand of the N positions, ascending (the FPS candidates).
  *   out_start (2*n_pairs) i32: the FPS start index in [0, n_cand).  out_valid (2*n_pairs) i32: points inside (or NULL).
- *   max_rows >= the longest scan; max(max_rows, N) <= usip_pair_max_scan_rows().
+ *   max_rows >= the longest scan, at most USIP_SUBSAMPLE_MAX_ROWS; N <= usip_pair_max_scan_rows(), the longest scan
+ *   the one-CTA kernel takes.  With max_rows <= usip_pair_max_scan_rows() both levels run in that kernel (one CTA per
+ *   cloud, keys in shared memory).  Above it the rows run in a kernel with one 8-CTA thread-block cluster per cloud that
+ *   regenerates the keys in every pass; the selection is defined as the N smallest (Philox key, row) pairs either way,
+ *   so out_rows and out_valid do not depend on which kernel ran.
  * usip_cloud_gather_candidates: out_pts (2*n_pairs, n_cand, 3) f32 = xyz of rows[c, cand[c, j]] of scan_of_cloud[c] --
  *   usip_fps_f32's input.
  * usip_pair_augment (augment(), :149-216, train mode only, then transform_pc_pytorch for dst, augmentation.py:199-248):
@@ -134,6 +138,7 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
 #define USIP_PAIR_TRANSLATION 16
 #define USIP_PAIR_ENU_TO_CAM 32
 #define USIP_PAIR_HEIGHT_SCALE 64
+#define USIP_SUBSAMPLE_MAX_ROWS 16777216           /* usip_cloud_subsample: the longest scan, 2^24 rows */
 int usip_pair_max_scan_rows(void);
 int usip_cloud_subsample(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud, int max_rows,
                          int n_pairs, int N, int n_cand, int use_radius, double radius, uint64_t seed, uint64_t step,

@@ -572,7 +572,10 @@ TEST_ROWS, TEST_SEED, TEST_N, TEST_M, TEST_B = 1300, 7500, 512, 32, 2
 TEST_CASES = {"plain": (61, 0.0), "noise": (62, 0.05)}      # name: (np / torch seed, noise sigma)
 
 
-def _golden_test_clouds(ref, module, make_loader, write_tree, out_name):
+def _golden_test_clouds(ref, module, make_loader, write_tree, out_name, sn_len=4, N=TEST_N, M=TEST_M, B=TEST_B,
+                        items=None, extra=None):
+    """module: the reference loader's module under evaluation/ or a dotted path; items: the loader indices, in order
+    (default all).  A rows draw of varying length (Redwood's remainder) is stored flat with its lengths."""
     import importlib
     import tempfile
     from torch.utils.data.dataloader import default_collate
@@ -584,9 +587,9 @@ def _golden_test_clouds(ref, module, make_loader, write_tree, out_name):
         import types
         sys.modules["PIL"] = types.ModuleType("PIL")
         sys.modules["PIL"].__dict__.update(Image=None, ImageMath=None)
-    tl = importlib.import_module("evaluation." + module)
-    out = {"tree/rows": np.int64(TEST_ROWS), "tree/seed": np.int64(TEST_SEED), "N": np.int64(TEST_N),
-           "M": np.int64(TEST_M), "batch_size": np.int64(TEST_B)}
+    tl = importlib.import_module(module if "." in module else "evaluation." + module)
+    out = {"tree/rows": np.int64(TEST_ROWS), "tree/seed": np.int64(TEST_SEED), "N": np.int64(N),
+           "M": np.int64(M), "batch_size": np.int64(B)}
     draws = []
     np_choice, np_randint = np.random.choice, np.random.randint
 
@@ -601,8 +604,10 @@ def _golden_test_clouds(ref, module, make_loader, write_tree, out_name):
         return r
     with tempfile.TemporaryDirectory() as root:
         write_tree(root)
-        opt = ref_shim.make_opt(input_pc_num=TEST_N, node_num=TEST_M, surface_normal_len=4)
+        opt = ref_shim.make_opt(input_pc_num=N, node_num=M, surface_normal_len=sn_len)
         loader = make_loader(tl, root, opt)
+        out.update(extra or {})                          # after make_loader, which may fill it
+        order = list(range(len(loader))) if items is None else list(items)
         np.random.choice, np.random.randint = choice, randint
         try:
             for name, (seed, sigma) in TEST_CASES.items():
@@ -610,8 +615,8 @@ def _golden_test_clouds(ref, module, make_loader, write_tree, out_name):
                 torch.manual_seed(seed)
                 del draws[:]
                 res = {"pc": [], "sn": [], "node": []}
-                for b0 in range(0, len(loader), TEST_B):
-                    batch = default_collate([loader[i] for i in range(b0, min(b0 + TEST_B, len(loader)))])
+                for b0 in range(0, len(order), B):
+                    batch = default_collate([loader[i] for i in order[b0:b0 + B]])
                     pc = batch[0]
                     if sigma:
                         pc = pc + torch.randn(pc.size()) * sigma
@@ -621,10 +626,14 @@ def _golden_test_clouds(ref, module, make_loader, write_tree, out_name):
                 out[name + "/noise_sigma"] = np.float64(sigma)
                 for k, v in res.items():
                     out[name + "/" + k] = np.concatenate(v)
-                out[name + "/rows"] = np.stack(draws[0::3]).astype(np.int32)
+                if len({len(r) for r in draws[0::3]}) == 1:
+                    out[name + "/rows"] = np.stack(draws[0::3]).astype(np.int32)
+                else:
+                    out[name + "/rows_flat"] = np.concatenate(draws[0::3]).astype(np.int32)
+                    out[name + "/rows_len"] = np.array([len(r) for r in draws[0::3]], dtype=np.int32)
                 out[name + "/cand"] = np.stack(draws[1::3]).astype(np.int32)
                 out[name + "/start"] = np.array(draws[2::3], dtype=np.int32)
-                print(out_name, name, {k: out[name + "/" + k].shape for k in ("pc", "sn", "node", "rows", "cand")})
+                print(out_name, name, {k: out[name + "/" + k].shape for k in ("pc", "sn", "node", "cand")})
         finally:
             np.random.choice, np.random.randint = np_choice, np_randint
     np.savez_compressed(os.path.join(OUT, out_name), **out)
@@ -653,6 +662,60 @@ def golden_oxford_test(ref):
         lambda root: write_synthetic_oxford_test(root, TEST_OX_NUMBERS, TEST_ROWS, TEST_OX_PAIRS,
                                                  os.path.join(root, "groundtruths.txt"), seed=TEST_SEED),
         "oxford_test_clouds.npz")
+
+
+# The rotated ModelNet40, Redwood and 3DMatch test loaders on synthetic trees, as above.  ModelNet: the reference
+# hard-codes 2468 objects, so the tree has MN_TEST_K of them and items 0..k-1 and 2468..2468+k-1 are drawn.  Redwood:
+# the reference's 207 frames, small, some shorter than N (taken whole, then a remainder).  3DMatch: every scene with
+# frame numbers out of order on disk; the reference's os.listdir order is recorded as `listing/<scene>`.
+MN_TEST_K, MN_TEST_N, MN_TEST_M, MN_TEST_B = 4, 512, 32, 4
+RW_TEST_N, RW_TEST_M, RW_TEST_B = 32, 8, 4
+M3_TEST_FRAMES, M3_TEST_N, M3_TEST_M, M3_TEST_B = (0, 10, 3), 256, 16, 4
+
+
+def redwood_test_rows(s, f):
+    """Rows of Redwood frame f of scene s in the synthetic tree: 5..80, so some frames are shorter than 32."""
+    return 5 + (37 * f + 11 * s) % 76
+
+
+def golden_modelnet_test(ref):
+    from usip_b200.evaluation import modelnet_test_loader as mtl
+    def write_tree(root):
+        names = ["obj_%04d" % i for i in range(MN_TEST_K)]
+        os.makedirs(os.path.join(root, "normal"))
+        mtl.write_synthetic_modelnet40_normal(os.path.join(root, "normal"), names, TEST_ROWS, seed=TEST_SEED)
+        mtl.write_rotated_modelnet(os.path.join(root, "normal"), os.path.join(root, "rotated_tree"), seed=TEST_SEED)
+    _golden_test_clouds(
+        ref, "data.modelnet_rotated_loader",
+        lambda tl, root, opt: tl.ModelNet_Rotated_Loader(os.path.join(root, "rotated_tree"), opt), write_tree,
+        "modelnet_test_clouds.npz", sn_len=3, N=MN_TEST_N, M=MN_TEST_M, B=MN_TEST_B,
+        items=list(range(MN_TEST_K)) + list(range(2468, 2468 + MN_TEST_K)), extra={"objects": np.int64(MN_TEST_K)})
+
+
+def golden_redwood_test(ref):
+    from usip_b200.evaluation import indoor_test_loader as itl
+    _golden_test_clouds(
+        ref, "redwood_loader", lambda tl, root, opt: tl.RedwoodLoader(os.path.join(root, "npy"), opt),
+        lambda root: itl.write_synthetic_redwood(os.path.join(root, "npy"), os.path.join(root, "gt"),
+                                                 redwood_test_rows, {}, seed=TEST_SEED),
+        "redwood_test_clouds.npz", N=RW_TEST_N, M=RW_TEST_M, B=RW_TEST_B)
+
+
+def golden_3dmatch_test(ref):
+    from usip_b200.evaluation import indoor_test_loader as itl
+    listing = {}
+    def make_loader(tl, root, opt):
+        loader = tl.Match3DEvalLoader(os.path.join(root, "npy"), opt)
+        for s in itl.MATCH3D_SCENES:
+            listing["listing/" + s] = np.array([os.path.basename(d[0]) for d in loader.dataset
+                                                if os.path.basename(os.path.dirname(d[0])) == s])
+        return loader
+    _golden_test_clouds(
+        ref, "data.match3d_eval_loader", make_loader,
+        lambda root: itl.write_synthetic_3dmatch(os.path.join(root, "npy"),
+                                                 {s: M3_TEST_FRAMES for s in itl.MATCH3D_SCENES}, TEST_ROWS, {},
+                                                 seed=TEST_SEED),
+        "3dmatch_test_clouds.npz", N=M3_TEST_N, M=M3_TEST_M, B=M3_TEST_B, extra=listing)
 
 
 def main():

@@ -13,7 +13,11 @@
 // cloud c is drawn from: the detector names every pair's scan twice (both sides subsample the same scan), the
 // descriptor names the anchor's and the positive's.  The Philox counters depend on c only, so the mapping changes no
 // random number.
+#include <cooperative_groups.h>
+
 #include "common.cuh"
+
+namespace cg = cooperative_groups;
 
 namespace usip {
 
@@ -72,11 +76,40 @@ __device__ __forceinline__ uint64_t block_exclusive_scan_u64(uint64_t v, uint64_
   return r;
 }
 
+// The subset's sort key of point i of cloud c: 31 random bits, so that no drawable point carries the sentinel, or
+// PG_SENTINEL when the point may not be drawn.  Both subset kernels draw through this one expression.
+__device__ __forceinline__ uint32_t pg_subset_key(bool ok, uint64_t seed, uint64_t step, int c, int i, int purpose) {
+  return ok ? (pg_random(seed, step, c, i, purpose, 0).x >> 1) : PG_SENTINEL;
+}
+
+// One radix digit: warp 0 finds the bin of hist[256] that holds the rem-th smallest key and writes it to s_ctl[0] and
+// the rank inside that bin to s_ctl[1].  The caller synchronises before reading s_ctl.
+__device__ __forceinline__ void pg_radix_pick(const uint32_t* hist, uint32_t rem, uint32_t* s_ctl) {
+  const int lane = threadIdx.x & 31;
+  uint32_t loc[8], s = 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) { loc[j] = hist[lane * 8 + j]; s += loc[j]; }
+  uint32_t inc = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  uint32_t c = inc - s;
+  if (c < rem && rem <= inc) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (c < rem && rem <= c + loc[j]) { s_ctl[0] = (uint32_t)(lane * 8 + j); s_ctl[1] = rem - c; }
+      c += loc[j];
+    }
+  }
+}
+
 // The `need` smallest (key, index) pairs among the keys != PG_SENTINEL: returns the threshold key T and how many of the
 // keys equal to T are taken (the lowest indices).  Four 8-bit radix passes over shared memory.  1 <= need <= #eligible.
 __device__ void pg_radix_threshold(const uint32_t* key, int n, int need, uint32_t* hist, uint32_t* s_ctl,
                                    uint32_t& T, int& take) {
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x;
   uint32_t prefix = 0, pmask = 0, rem = (uint32_t)need;
   for (int shift = 24; shift >= 0; shift -= 8) {
     for (int i = tid; i < 256; i += blockDim.x) hist[i] = 0;
@@ -86,25 +119,7 @@ __device__ void pg_radix_threshold(const uint32_t* key, int n, int need, uint32_
       if (k != PG_SENTINEL && (k & pmask) == prefix) atomicAdd(&hist[(k >> shift) & 255u], 1u);
     }
     __syncthreads();
-    if (tid < 32) {
-      uint32_t loc[8], s = 0;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { loc[j] = hist[lane * 8 + j]; s += loc[j]; }
-      uint32_t inc = s;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-      }
-      uint32_t c = inc - s;
-      if (c < rem && rem <= inc) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (c < rem && rem <= c + loc[j]) { s_ctl[0] = (uint32_t)(lane * 8 + j); s_ctl[1] = rem - c; }
-          c += loc[j];
-        }
-      }
-    }
+    if (tid < 32) pg_radix_pick(hist, rem, s_ctl);
     __syncthreads();
     prefix |= s_ctl[0] << shift;
     pmask |= 0xffu << shift;
@@ -139,11 +154,10 @@ pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __rest
   const int n = level == 0 ? (int)(offsets[scan + 1] - row0) : N;
   const float* base = scans + row0 * C;
 
-  // keys: 31 random bits, so that no drawable point carries the sentinel
   int my_valid = 0;
   for (int i = tid; i < n; i += blockDim.x) {
     const bool ok = level != 0 || !use_radius || pg_inside(base + (int64_t)i * C, radius);
-    key[i] = ok ? (pg_random(seed, step, c, i, level == 0 ? PURPOSE_ROWS : PURPOSE_CAND, 0).x >> 1) : PG_SENTINEL;
+    key[i] = pg_subset_key(ok, seed, step, c, i, level == 0 ? PURPOSE_ROWS : PURPOSE_CAND);
     my_valid += ok;
   }
   const uint64_t nvalid_excl = block_exclusive_scan_u64((uint64_t)my_valid, s_warp);
@@ -198,6 +212,126 @@ pair_subset_kernel(const float* __restrict__ scans, int C, const int64_t* __rest
     }
     ++vr;
   }
+}
+
+// Level 0 of a batch whose longest scan exceeds what pair_subset_kernel keeps in shared memory: one thread-block
+// cluster of PG_CLUSTER CTAs per cloud, CTA r owning the contiguous slice [r*per, (r+1)*per) of the scan's rows.  No
+// key is stored: every pass regenerates it with pg_subset_key, so the rows (the N smallest (key, row) pairs, the tile
+// path, rows 0 without a valid point) and out_valid are exactly pair_subset_kernel's for the same (seed, step, cloud).
+// The CTAs exchange their counts and radix histograms through distributed shared memory.  A slice has at most
+// USIP_SUBSAMPLE_MAX_ROWS / PG_CLUSTER = 2^21 rows, so the counts are kept in 32 bits.
+constexpr int PG_CLUSTER = 8;                      // the portable cluster size
+
+__global__ void __cluster_dims__(PG_CLUSTER, 1, 1) __launch_bounds__(PG_THREADS)
+pair_subset_cluster_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
+                           const int32_t* __restrict__ scan_of_cloud, int use_radius, double radius, int N,
+                           uint64_t seed, uint64_t step, int32_t* __restrict__ out_rows,
+                           int32_t* __restrict__ out_valid) {
+  cg::cluster_group cluster = cg::this_cluster();
+  __shared__ uint32_t hist[256];
+  __shared__ uint32_t s_ctl[2];
+  __shared__ uint32_t s_part[3];                   // this CTA's (valid, less, equal) counts, read by the others
+  __shared__ uint64_t s_warp[32];
+  const int rank = (int)cluster.block_rank(), c = blockIdx.x / PG_CLUSTER, tid = threadIdx.x;
+  const int scan = scan_of_cloud[c];
+  const int64_t row0 = offsets[scan];
+  const int n = (int)(offsets[scan + 1] - row0);
+  const float* base = scans + row0 * C;
+  const int per = (n + PG_CLUSTER - 1) / PG_CLUSTER;
+  const int lo = min(n, rank * per), hi = min(n, lo + per);
+  auto inside = [&](int i) { return !use_radius || pg_inside(base + (int64_t)i * C, radius); };
+  auto key_of = [&](int i) { return pg_subset_key(inside(i), seed, step, c, i, PURPOSE_ROWS); };
+
+  // pass 1: valid rows, in the whole scan and below this slice
+  uint32_t my_valid = 0;
+  for (int i = lo + tid; i < hi; i += blockDim.x) my_valid += inside(i);
+  const uint64_t vex = block_exclusive_scan_u64(my_valid, s_warp);
+  if (tid == blockDim.x - 1) s_part[0] = (uint32_t)(vex + my_valid);
+  cluster.sync();
+  int nvalid = 0, valid_base = 0;
+  for (int r = 0; r < PG_CLUSTER; ++r) {
+    const int v = (int)*cluster.map_shared_rank(&s_part[0], r);
+    nvalid += v;
+    valid_base += r < rank ? v : 0;
+  }
+
+  int tiles = 0, need = N;
+  if (out_valid && rank == 0 && tid == 0) out_valid[c] = nvalid;
+  if (nvalid == 0) {                               // nothing to draw from: every row is 0 (see the header)
+    need = 0;
+    for (int i = rank * blockDim.x + tid; i < N; i += PG_CLUSTER * blockDim.x) out_rows[(int64_t)c * N + i] = 0;
+  } else if (nvalid < N) {                         // kitti_detector_loader.py:129-133
+    tiles = max(1, (N + nvalid - 1) / nvalid - 1);
+    need = N - tiles * nvalid;
+  }
+
+  // pass 2: four 8-bit radix passes; every CTA sums the eight histograms in rank order and picks the same digit
+  uint32_t prefix = 0, pmask = 0, rem = (uint32_t)need;
+  if (need > 0) {
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      for (int i = tid; i < 256; i += blockDim.x) hist[i] = 0;
+      __syncthreads();
+      for (int i = lo + tid; i < hi; i += blockDim.x) {
+        const uint32_t k = key_of(i);
+        if (k != PG_SENTINEL && (k & pmask) == prefix) atomicAdd(&hist[(k >> shift) & 255u], 1u);
+      }
+      cluster.sync();                              // every slice's histogram is complete
+      uint32_t sum = 0;
+      if (tid < 256)
+        for (int r = 0; r < PG_CLUSTER; ++r) sum += cluster.map_shared_rank(hist, r)[tid];
+      cluster.sync();                              // no CTA clears its histogram while another still reads it
+      if (tid < 256) hist[tid] = sum;
+      __syncthreads();
+      if (tid < 32) pg_radix_pick(hist, rem, s_ctl);
+      __syncthreads();
+      prefix |= s_ctl[0] << shift;
+      pmask |= 0xffu << shift;
+      rem = s_ctl[1];
+    }
+  }
+  const uint32_t T = prefix;
+  const int take = (int)rem;
+
+  // pass 3: ordered emission.  Inside the CTA each thread owns a contiguous chunk of the slice (block scans of the
+  // (less, equal) and valid counts); the CTA's base is the sum over the lower ranks.
+  const int len = hi - lo, chunk = (len + blockDim.x - 1) / blockDim.x;
+  const int i0 = lo + min(len, tid * chunk), i1 = lo + min(len, tid * chunk + chunk);
+  uint64_t lt_eq = 0;
+  uint32_t nv = 0;
+  for (int i = i0; i < i1; ++i) {
+    const uint32_t k = key_of(i);
+    if (k == PG_SENTINEL) continue;
+    lt_eq += (need > 0 && k < T) ? 1ull : 0ull;
+    lt_eq += (need > 0 && k == T) ? (1ull << 32) : 0ull;
+    ++nv;
+  }
+  const uint64_t ex = block_exclusive_scan_u64(lt_eq, s_warp);
+  const uint64_t ex_v = block_exclusive_scan_u64(nv, s_warp);
+  if (tid == blockDim.x - 1) {
+    s_part[1] = (uint32_t)(ex + lt_eq);
+    s_part[2] = (uint32_t)((ex + lt_eq) >> 32);
+  }
+  cluster.sync();
+  int less = (int)(uint32_t)ex, eq = (int)(ex >> 32), vr = valid_base + (int)ex_v;
+  for (int r = 0; r < rank; ++r) {
+    less += (int)*cluster.map_shared_rank(&s_part[1], r);
+    eq += (int)*cluster.map_shared_rank(&s_part[2], r);
+  }
+  int32_t* out = out_rows + (int64_t)c * N;
+  const int sel_base = tiles * nvalid;
+  for (int i = i0; i < i1; ++i) {
+    const uint32_t k = key_of(i);
+    if (k == PG_SENTINEL) continue;
+    for (int t = 0; t < tiles; ++t) out[t * nvalid + vr] = i;
+    if (need > 0) {
+      if (k < T) out[sel_base + less + min(eq, take)] = i;
+      else if (k == T && eq < take) out[sel_base + less + eq] = i;
+      less += k < T;
+      eq += k == T;
+    }
+    ++vr;
+  }
+  cluster.sync();                                  // no CTA exits while another may still read its shared memory
 }
 
 // candidate points for FPS: pts[c, j, :] = xyz of row rows[c, cand[c, j]]; with z_scale, z is fl32(z * z_scale[c])
@@ -609,6 +743,7 @@ using namespace usip;
 
 static int pg_subset_smem(int n) { return n * (int)sizeof(uint32_t); }
 
+// the longest scan pair_subset_kernel keeps in shared memory (one 31-bit key per row); also the largest N
 extern "C" int usip_pair_max_scan_rows(void) {
   return (227 * 1024 - 4096) / (int)sizeof(uint32_t);
 }
@@ -621,16 +756,24 @@ extern "C" int usip_cloud_subsample(const float* scans, int C, const int64_t* of
   USIP_REQUIRE(scans && offsets && scan_of_cloud && out_rows && out_cand && out_start, "cloud_subsample: null pointer");
   USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N && max_rows > 0,
                "cloud_subsample: bad sizes");
-  USIP_REQUIRE(max(max_rows, N) <= usip_pair_max_scan_rows(),
-               "cloud_subsample: scan or N too large for shared memory");
+  USIP_REQUIRE(max_rows <= USIP_SUBSAMPLE_MAX_ROWS, "cloud_subsample: a scan may have at most 16777216 rows");
+  USIP_REQUIRE(N <= usip_pair_max_scan_rows(), "cloud_subsample: N too large for shared memory");
+  const bool one_cta = max_rows <= usip_pair_max_scan_rows();
   cudaError_t e = cudaFuncSetAttribute(pair_subset_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       pg_subset_smem(max(max_rows, N)));
+                                       pg_subset_smem(one_cta ? max(max_rows, N) : N));
   if (e != cudaSuccess) { set_last_error("cloud_subsample: smem attribute"); return (int)e; }
   cudaStream_t s = (cudaStream_t)stream;
-  pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(max_rows), s>>>(
-      scans, C, offsets, scan_of_cloud, 0, use_radius, radius, N, n_cand, seed, step, out_rows, out_cand, out_start,
-      out_valid);
-  int rc = check_launch("pair_subset_kernel(rows)");
+  int rc;
+  if (one_cta) {
+    pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(max_rows), s>>>(
+        scans, C, offsets, scan_of_cloud, 0, use_radius, radius, N, n_cand, seed, step, out_rows, out_cand, out_start,
+        out_valid);
+    rc = check_launch("pair_subset_kernel(rows)");
+  } else {
+    pair_subset_cluster_kernel<<<2 * n_pairs * PG_CLUSTER, PG_THREADS, 0, s>>>(
+        scans, C, offsets, scan_of_cloud, use_radius, radius, N, seed, step, out_rows, out_valid);
+    rc = check_launch("pair_subset_cluster_kernel(rows)");
+  }
   if (rc) return rc;
   pair_subset_kernel<<<2 * n_pairs, PG_THREADS, pg_subset_smem(N), s>>>(
       scans, C, offsets, scan_of_cloud, 1, 0, 0.0, N, n_cand, seed, step, out_rows, out_cand, out_start, out_valid);

@@ -54,22 +54,26 @@ def make_kitti_test_dataset(txt_root):
 
 class _TestCloudSource:
     """Batches of test clouds built on the device.  A subclass lists the scan files (`paths`), names each item's
-    keypoint file (`keypoint_path`) and the key its ground truth uses (`key`), and sets the FPS candidate divisor and
-    the frame flags.  `build(items)` -> (pc (B,3,N), sn (B,4,N), node (B,3,M)) f32, fresh tensors on the current
-    stream; nothing synchronises with the host."""
+    keypoint file (`keypoint_path`) and the key its ground truth uses (`key`), and sets the FPS candidate divisor, the
+    frame flags, the surface-normal length sn_len (columns 3:3+sn_len) and whether a scan may be shorter than
+    input_pc_num (allow_short: every row is taken t times, then a random remainder, as usip_cloud_subsample and
+    draw_subsample do).  `build(items)` -> (pc (B,3,N), sn (B,sn_len,N), node (B,3,M)) f32, fresh tensors on the
+    current stream; nothing synchronises with the host."""
 
     divisor = 4
     flags = 0
+    sn_len = TEST_SN_LEN
+    allow_short = False
 
     def __init__(self, paths, opt, device, seed, rng, batch_size):
-        if int(opt.surface_normal_len) != TEST_SN_LEN:
-            raise ValueError("surface_normal_len must be %d for the test loaders, got %d"
-                             % (TEST_SN_LEN, int(opt.surface_normal_len)))
+        if int(opt.surface_normal_len) != self.sn_len:
+            raise ValueError("surface_normal_len must be %d for this test loader, got %d"
+                             % (self.sn_len, int(opt.surface_normal_len)))
         if rng not in ("device", "numpy"):
             raise ValueError("rng must be 'device' or 'numpy'")
         self.opt, self.paths, self.rng, self.seed = opt, list(paths), rng, int(seed)
         self.device = torch.device(device if device is not None else "cuda")
-        self.N, self.M, self.S = int(opt.input_pc_num), int(opt.node_num), TEST_SN_LEN
+        self.N, self.M, self.S = int(opt.input_pc_num), int(opt.node_num), self.sn_len
         self.n_cand = int(self.N / self.divisor)
         if self.n_cand > FPS_MAX_CANDIDATES:
             raise ValueError("input_pc_num / %d = %d FPS candidates; usip_fps_f32 takes at most %d"
@@ -92,11 +96,11 @@ class _TestCloudSource:
         raise NotImplementedError
 
     def load(self, items):
-        """The items' scans as (Ns, C) float32 arrays; a scan shorter than input_pc_num raises ValueError (the
-        reference draws its rows without replacement and has no fill)."""
+        """The items' scans as (Ns, C) float32 arrays.  Unless allow_short, a scan shorter than input_pc_num raises
+        ValueError (the reference draws its rows without replacement and has no fill); an empty scan always does."""
         arrs = [load_scan_npy(self.paths[i], self.S) for i in items]
         for i, a in zip(items, arrs):
-            if len(a) < self.N:
+            if len(a) == 0 or (len(a) < self.N and not self.allow_short):
                 raise ValueError("scan %s (%s) has %d rows; input_pc_num = %d rows are drawn without replacement"
                                  % (self.key(i), self.paths[i], len(a), self.N))
         if len({a.shape[1] for a in arrs}) != 1:

@@ -1,5 +1,6 @@
 """Keypoint repeatability on the GPU: evaluation/save_keypoints.py (detection, NMS, sigma-sorted top K) followed by
-evaluation/matlab/eval_repeatability/eval_rep.m (the score), for the KITTI and Oxford test sets.
+evaluation/matlab/eval_repeatability/eval_rep.m (the score), for the KITTI, Oxford, rotated ModelNet40, Redwood and
+3DMatch test sets.
 
 One pass of the detector over the test set gives the whole keypoint-count sweep: every scan's keypoints, sigmas and
 selection order stay on the device, each K reads a prefix of that order, and one launch of usip_repeatability_f64
@@ -16,6 +17,9 @@ inliers = #{anchor keypoints whose nearest positive keypoint is closer than inli
 repeatability = inliers / n_anc.  KITTI: keypoints leave the camera frame with inv(Tr) (cam2velodyne.m), Tr from
 <calib_root>/<seq>/calib.txt; pairs from <txt_root>/<seq>/correct_gt.txt.  Oxford: coord_cam2enu.m, (x, y, z) ->
 (x, z, -y); pairs from groundtruths.txt.  T_gt = [quat2rotm(q), t] with q normalised first, as MATLAB does.
+ModelNet, Redwood and 3DMatch (eval_rep.m:87-126): F_a = F_p = I.  ModelNet pairs object i of original/ with object i
+of rotated/, T_gt = [R, 0] from modelnet_info.mat; Redwood and 3DMatch pair the fragments of every gt.log line, T_gt =
+the top three rows of its 4x4.  eval_rep.m's apply_transform(x, T) = [x 1] * T' is exactly the map applied here.
 
 Deliberate deviations from the reference:
   * save_keypoints.py:348-349 overwrites desired_keypoint_num with the keypoint count of the first scan that has fewer
@@ -24,6 +28,7 @@ Deliberate deviations from the reference:
     in another order (as in save_keypoints.select_keypoints).
   * Every run draws its subsamples from a seed (or replays np.random in parity mode) instead of a fresh random state.
   * The homogeneous step of cam2velodyne.m is dropped: the keypoints go through the top three rows of inv(Tr).
+  * 3DMatch fragments are taken in frame order, not os.listdir's (indoor_test_loader.py).
 """
 import argparse
 import json
@@ -35,7 +40,9 @@ import torch
 
 from usip_b200 import ops
 
+from .indoor_test_loader import MATCH3D_SCENES, REDWOOD_SCENES, Match3DTestLoader, RedwoodTestLoader
 from .kitti_test_loader import KittiTestLoader
+from .modelnet_test_loader import ModelNetRotatedTestLoader, eul2rotm, write_rotated_modelnet  # noqa: F401
 from .oxford_test_loader import OxfordTestLoader
 from .save_keypoints import write_keypoints_bin
 
@@ -95,6 +102,42 @@ def read_kitti_calib(path):
             out[parts[0].rstrip(":")] = np.concatenate([np.array(parts[1:13], dtype=np.float64).reshape(3, 4),
                                                         [[0, 0, 0, 1.0]]])
     return out
+
+
+def read_gt_log(path):
+    """mrLoadLog.m: a stream of whitespace-separated numbers, three integers (anc, pos, and a count) then 16 numbers
+    forming a row-major 4x4, repeated until fewer than three integers remain -> (anc (n,) int64, pos (n,) int64,
+    T (n, 3, 4) float64, the top three rows)."""
+    with open(path) as f:
+        tok = f.read().split()
+    anc, pos, T = [], [], []
+    at = 0
+    while at + 3 <= len(tok):
+        try:
+            head = [int(t) for t in tok[at:at + 3]]
+        except ValueError:
+            break
+        m = tok[at + 3:at + 19]
+        if len(m) != 16:
+            raise ValueError("%s: the entry for (%d, %d) has %d of its 16 matrix values" % (path, head[0], head[1],
+                                                                                             len(m)))
+        anc.append(head[0]); pos.append(head[1])
+        T.append(np.array(m, dtype=np.float64).reshape(4, 4)[:3])
+        at += 19
+    return (np.array(anc, dtype=np.int64), np.array(pos, dtype=np.int64),
+            np.array(T, dtype=np.float64).reshape(-1, 3, 4))
+
+
+def read_modelnet_info(path):
+    """modelnet_info.mat (rotate_modelnet_dateset.m): the cell array modelnet_info, one row per object; column 3 is
+    T = [R, 0] -> (n, 3, 4) float64.  scipy reads MATLAB files up to v7; a v7.3 (HDF5) file raises ValueError."""
+    import scipy.io
+    try:
+        info = scipy.io.loadmat(path)["modelnet_info"]
+    except NotImplementedError as e:
+        raise ValueError("%s is a MATLAB v7.3 (HDF5) file, which scipy.io cannot read; re-save it with "
+                         "save(..., '-v7')" % path) from e
+    return np.stack([np.asarray(info[i, 2], dtype=np.float64).reshape(3, 4) for i in range(info.shape[0])])
 
 
 def cam_to_velodyne(Tr):
@@ -226,7 +269,8 @@ class Repeatability:
         return self.keypoints[i][:, self.order[i, :n].long()].t().contiguous()
 
     def write_keypoint_tree(self, out_dir, K):
-        """The reference's keypoint files for K (save_keypoints.py:367-393): KITTI %02d/%06d.bin, Oxford %d.bin."""
+        """The reference's keypoint files for K (save_keypoints.py:367-393): KITTI %02d/%06d.bin, Oxford %d.bin,
+        ModelNet original|rotated/%d.bin, Redwood and 3DMatch <scene>/%d.bin."""
         if self.keypoints is None:
             raise RuntimeError("detect() first")
         for i in range(len(self.source)):
@@ -267,10 +311,76 @@ class OxfordRepeatability(Repeatability):
         super().__init__(source, keys, np.array(frames).reshape(-1, 3, 3, 4))
 
 
+class _IdentityFrameRepeatability(Repeatability):
+    """Pairs whose keypoints are already in one frame up to T_gt: F_a = F_p = I (eval_rep.m:87-126)."""
+
+    def __init__(self, source, pair_keys, T_gt):
+        T_gt = np.asarray(T_gt, dtype=np.float64).reshape(-1, 3, 4)
+        I = np.broadcast_to(np.eye(3, 4), T_gt.shape)
+        super().__init__(source, pair_keys, np.stack([I, I, T_gt], axis=1))
+
+
+class ModelNetRepeatability(_IdentityFrameRepeatability):
+    """Rotated ModelNet40: scans from ModelNetRotatedTestLoader(root, opt), one pair (original i, rotated i) per row of
+    <root>/modelnet_info.mat (or info_path), T_gt = its [R, 0]."""
+
+    dataset = "modelnet"
+
+    def __init__(self, root, opt, device=None, seed=0, rng="device", batch_size=4, info_path=None):
+        T = read_modelnet_info(info_path or os.path.join(root, "modelnet_info.mat"))
+        source = ModelNetRotatedTestLoader(root, opt, device, seed, rng, batch_size, n=len(T))
+        keys = [(("original", i), ("rotated", i)) for i in range(len(T))]
+        super().__init__(source, keys, T)
+
+
+def _gt_log_pairs(scenes, log_path):
+    keys, T = [], []
+    for scene in scenes:
+        anc, pos, t = read_gt_log(log_path(scene))
+        keys += [((scene, int(a)), (scene, int(p))) for a, p in zip(anc, pos)]
+        T.append(t)
+    return keys, np.concatenate(T) if T else np.zeros((0, 3, 4))
+
+
+class RedwoodRepeatability(_IdentityFrameRepeatability):
+    """Redwood: scans from RedwoodTestLoader(npy_root, opt) (numpy_gt_normal), pairs and T_gt from every scene's
+    <gt_root>/original/<scene>-evaluation/gt.log (build_redwood_dataset.m)."""
+
+    dataset = "redwood"
+
+    def __init__(self, npy_root, gt_root, opt, device=None, seed=0, rng="device", batch_size=8,
+                 scenes=REDWOOD_SCENES):
+        source = RedwoodTestLoader(npy_root, opt, device, seed, rng, batch_size, scenes)
+        keys, T = _gt_log_pairs([s for s, _ in source.scenes],
+                                lambda s: os.path.join(gt_root, "original", "%s-evaluation" % s, "gt.log"))
+        super().__init__(source, keys, T)
+
+
+class Match3DRepeatability(_IdentityFrameRepeatability):
+    """3DMatch: scans from Match3DTestLoader(root, opt) (3DMatch_eval_npy), pairs and T_gt from every scene's
+    <gt_root>/<scene>-evaluation/gt.log, gt_root = root by default (build_3dmatch_dataset.m)."""
+
+    dataset = "3dmatch"
+
+    def __init__(self, root, opt, device=None, seed=0, rng="device", batch_size=8, gt_root=None, files=None,
+                 scenes=MATCH3D_SCENES):
+        source = Match3DTestLoader(root, opt, device, seed, rng, batch_size, files, scenes)
+        keys, T = _gt_log_pairs(source.scenes,
+                                lambda s: os.path.join(gt_root or root, "%s-evaluation" % s, "gt.log"))
+        super().__init__(source, keys, T)
+
+
 # ----------------------------------------------------------------------------------------------- command line
+DATASETS = ("kitti", "oxford", "modelnet", "redwood", "3dmatch")
+DEFAULT_BATCH_SIZE = {"modelnet": 4}              # 8 for the others
+
+
 def detector_opt(dataset, **over):
-    """The reference's KITTI / Oxford detector options (kitti/options_detector.py, oxford/options_detector.py) for
-    evaluation on cuda:0."""
+    """The reference's detector options for evaluation on cuda:0: kitti/ and oxford/options_detector.py; modelnet/
+    (modelnet), scenenn/ (redwood) and match3d/options_detector.py (3dmatch).  loss_sigma_lower_bound enters the
+    sigmas, and so the keypoint order."""
+    if dataset not in DATASETS:
+        raise ValueError("dataset must be one of %s, got %r" % (", ".join(DATASETS), dataset))
     o = types.SimpleNamespace(
         gpu_ids=[0], device=torch.device("cuda:0"), scene="outdoor", batch_size=8, input_pc_num=16384,
         surface_normal_len=4, node_num=512, k=1, node_knn_k_1=16, activation="relu", normalization="batch",
@@ -278,6 +388,13 @@ def detector_opt(dataset, **over):
         random_pc_dropout_lower_limit=1.0, keypoint_on_pc_type="point_to_point",
         keypoint_on_pc_alpha=0.01 if dataset == "kitti" else 1.0, rot_3d=False, rot_horizontal=True,
         rot_perturbation=False, translation_perturbation=False, checkpoints_dir="./checkpoints")
+    if dataset == "modelnet":
+        o.__dict__.update(scene="object", batch_size=4, input_pc_num=5000, surface_normal_len=3, node_knn_k_1=32,
+                          loss_sigma_lower_bound=1e-4, keypoint_on_pc_alpha=1.0, rot_3d=True, rot_horizontal=False)
+    elif dataset in ("redwood", "3dmatch"):
+        o.__dict__.update(input_pc_num=10240, node_knn_k_1=32, loss_sigma_lower_bound=1e-4,
+                          keypoint_on_pc_alpha=100.0 if dataset == "redwood" else 10.0, rot_3d=True,
+                          rot_horizontal=False)
     o.__dict__.update(over)
     return o
 
@@ -299,36 +416,59 @@ def load_detector_checkpoint(model, path):
 def main(argv=None):
     ap = argparse.ArgumentParser(prog="python -m usip_b200.evaluation.repeatability",
                                  description="Keypoint repeatability of a trained detector (save_keypoints.py + "
-                                             "eval_rep.m) on the KITTI or Oxford test set.")
-    ap.add_argument("dataset", choices=("kitti", "oxford"))
+                                             "eval_rep.m) on the KITTI, Oxford, rotated ModelNet40, Redwood or 3DMatch "
+                                             "test set.")
+    ap.add_argument("dataset", choices=DATASETS)
     ap.add_argument("--checkpoint", required=True, help="detector state dict (the reference's *_net_detector.pth)")
     ap.add_argument("--txt-root", help="kitti: the folder of <seq>/groundtruths.txt and <seq>/correct_gt.txt")
     ap.add_argument("--numpy-root", help="kitti: the folder of <seq>/np_0.20_20480_r90_sn/%%06d.npy")
     ap.add_argument("--calib-root", help="kitti: the folder of <seq>/calib.txt")
-    ap.add_argument("--root", help="oxford: the folder of test_models_20k_np_nofilter/")
-    ap.add_argument("--gt", help="oxford: groundtruths.txt")
+    ap.add_argument("--root", help="oxford: the folder of test_models_20k_np_nofilter/; modelnet: the rotated tree "
+                                   "(original/, rotated/, modelnet_info.mat); redwood: numpy_gt_normal/; 3dmatch: "
+                                   "3DMatch_eval_npy/")
+    ap.add_argument("--gt", help="oxford: groundtruths.txt; modelnet: modelnet_info.mat (default <root>/...)")
+    ap.add_argument("--gt-root", help="redwood: the folder of original/<scene>-evaluation/gt.log; 3dmatch: the folder "
+                                      "of <scene>-evaluation/gt.log (default --root)")
     ap.add_argument("--keypoint-nums", type=int, nargs="+", default=list(DEFAULT_KEYPOINT_NUMS))
     ap.add_argument("--nms-radius", type=float, default=0.0)
     ap.add_argument("--inlier-radius", type=float, default=DEFAULT_INLIER_RADIUS)
     ap.add_argument("--noise-sigma", type=float, default=0.0)
-    ap.add_argument("--batch-size", type=int, default=8)
+    ap.add_argument("--batch-size", type=int, help="default 4 for modelnet, 8 otherwise")
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--input-pc-num", type=int, default=16384)
+    ap.add_argument("--input-pc-num", type=int, help="default: the dataset's (16384, 5000 for modelnet, 10240 for "
+                                                     "redwood and 3dmatch)")
     ap.add_argument("--node-num", type=int, default=512)
     ap.add_argument("--write-keypoints", metavar="DIR", help="also write the .bin tree of the largest K")
     ap.add_argument("--json", metavar="OUT", help="write the summary as JSON")
     a = ap.parse_args(argv)
     check_sweep(a.keypoint_nums, a.inlier_radius)
     from usip_b200.models.keypoint_detector import ModelDetector
-    opt = detector_opt(a.dataset, batch_size=a.batch_size, input_pc_num=a.input_pc_num, node_num=a.node_num)
+    bs = a.batch_size or DEFAULT_BATCH_SIZE.get(a.dataset, 8)
+    over = {"batch_size": bs, "node_num": a.node_num}
+    if a.input_pc_num:
+        over["input_pc_num"] = a.input_pc_num
+    opt = detector_opt(a.dataset, **over)
+    kw = {"seed": a.seed, "batch_size": bs}
     if a.dataset == "kitti":
         if not (a.txt_root and a.numpy_root and a.calib_root):
             ap.error("kitti needs --txt-root, --numpy-root and --calib-root")
-        ev = KittiRepeatability(a.txt_root, a.numpy_root, a.calib_root, opt, seed=a.seed, batch_size=a.batch_size)
-    else:
+        ev = KittiRepeatability(a.txt_root, a.numpy_root, a.calib_root, opt, **kw)
+    elif a.dataset == "oxford":
         if not (a.root and a.gt):
             ap.error("oxford needs --root and --gt")
-        ev = OxfordRepeatability(a.root, a.gt, opt, seed=a.seed, batch_size=a.batch_size)
+        ev = OxfordRepeatability(a.root, a.gt, opt, **kw)
+    elif a.dataset == "modelnet":
+        if not a.root:
+            ap.error("modelnet needs --root")
+        ev = ModelNetRepeatability(a.root, opt, info_path=a.gt, **kw)
+    elif a.dataset == "redwood":
+        if not (a.root and a.gt_root):
+            ap.error("redwood needs --root and --gt-root")
+        ev = RedwoodRepeatability(a.root, a.gt_root, opt, **kw)
+    else:
+        if not a.root:
+            ap.error("3dmatch needs --root")
+        ev = Match3DRepeatability(a.root, opt, gt_root=a.gt_root, **kw)
     model = ModelDetector(opt)
     load_detector_checkpoint(model, a.checkpoint)
     res = ev.run(model, a.keypoint_nums, a.nms_radius, a.inlier_radius, a.noise_sigma)

@@ -141,6 +141,7 @@ def fps(pts, start, k, want_nodes=True):
 PAIR_TRAIN, PAIR_ROT_HORIZONTAL, PAIR_ROT_3D, PAIR_ROT_PERTURBATION, PAIR_TRANSLATION = 1, 2, 4, 8, 16
 PAIR_ENU_TO_CAM, PAIR_HEIGHT_SCALE = 32, 64      # Oxford: camera frame first; detector height scale = params[:, 44]
 PAIR_PARAM_STRIDE = 48                           # detector: doubles per pair
+SUBSAMPLE_MAX_ROWS = 1 << 24                     # cloud_subsample: the longest scan (USIP_SUBSAMPLE_MAX_ROWS)
 DESC_PARAM_STRIDE = 32                           # descriptor: doubles per cloud
 
 
@@ -165,7 +166,8 @@ def _req_jitter(jit_pc, jit_sn, jit_node):
 def cloud_subsample(scans, offsets, scan_of_cloud, max_rows, N, n_cand, radius=None, seed=0, step=0):
     """Device-mode subsets of 2B clouds.  scans [T, C] f32, offsets (n_scans+1,) i64, scan_of_cloud (2B,) i32 the scan
     of every cloud -> rows (2B, N) i32, cand (2B, n_cand) i32, start (2B,) i32, valid (2B,) i32 (points inside the
-    radius)."""
+    radius).  max_rows (the longest scan) may be up to SUBSAMPLE_MAX_ROWS; scans longer than pair_max_scan_rows() run
+    in the cluster kernel, which selects the same rows.  N <= pair_max_scan_rows()."""
     _req_scans(scans, offsets, scan_of_cloud)
     B, dev = scan_of_cloud.shape[0] // 2, scans.device
     rows = torch.empty((2 * B, int(N)), dtype=i32, device=dev)
