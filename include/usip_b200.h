@@ -255,6 +255,50 @@ int usip_ransac_rt_f64(const float* xyz, const int32_t* count, int n_scans, int 
 /* the uniforms of trials 0..T-1 of usip_ransac_rt_f64's Philox stream -> out (T, 3) f64 */
 int usip_ransac_uniforms(uint64_t seed, int T, double* out, void* stream);
 
+/* Information matrix of the registration      evaluation/matlab/eval_indoor/3dmatch/register2Fragments.m:77-88.
+ * The inputs of usip_ransac_rt_f64 (same values: the matches, the trial sweep, threshold, seed and uniforms), plus its
+ * best_trial and status (P, nK, nT) i32.  For each (pair, K, budget) with status 0 the best trial's model is derived
+ * again from the same uniforms (sample and 3-point fit as in usip_ransac_rt_f64; npts == 3: all three matches), its
+ * inliers are taken in ascending match order, and info = sum over them, in that order, of A^T A with
+ * A = [I3 | [[0, 2z, -2y], [-2z, 0, 2x], [2y, -2x, 0]]], (x, y, z) = F_a * the anchor row (fragment 1's keypoint);
+ * entry (r, c) of A^T A is ((A0r A0c + A1r A1c) + A2r A2c), all fp64 without contraction.  n_info = the inlier count,
+ * which equals usip_ransac_rt_f64's n_inliers.  status != 0: info zero and n_info 0 (register2Fragments.m's catch: no
+ * inliers).  A status-0 entry whose best trial lies outside the stream or does not fit the matches: info zero, n_info -1.
+ * -> info (P, nK, nT, 6, 6) f64 row-major, n_info (P, nK, nT) i32. */
+int usip_ransac_info_f64(const float* xyz, const int32_t* count, int n_scans, int L, const int32_t* pairs,
+                         const double* frames, int P, int nK, const int32_t* matches, const int32_t* n_matches, int cap,
+                         const int32_t* trials, int nT, double threshold, uint64_t seed, const double* uniforms,
+                         const int32_t* best_trial, const int32_t* status, double* info, int32_t* n_info, void* stream);
+
+/* Fragment overlap      register2Fragments.m:134-137 (ratioAligned(1)), for J (fragment a, fragment b, map) jobs at once.
+ * xyz (sum of rows, 3) f32: every fragment's rows packed (columns 0:3 of its .npy), device; offsets (n_frags + 1) i64,
+ * HOST memory, offsets[0] = 0, fragment f = rows [offsets[f], offsets[f+1]); jobs (J, 2) i32, HOST memory: fragment a
+ * (the reference's fragment 1) and fragment b; Rt (J, 3, 4) f64, device: x_a = R x_b + t, as usip_ransac_rt_f64 returns
+ * it.  -> hits (J,) i32, device.
+ *   Rule: every point of b is mapped in fp64 without contraction, ((r0 x + r1 y) + r2 z) + t per row, then rounded once
+ *   to fp32: b'.  A point p of a is a hit iff some b' has sqrtf(d2) < radius, d2 = (dx dx + dy dy) + dz dz in fp32
+ *   round-to-nearest without FMA, radius fp32; tested as d2 <= t_lim, t_lim the largest fp32 with sqrtf(t_lim) <
+ *   radius, found on the host.  A point with a non-finite coordinate, in a or in b, is never a hit (it still counts in
+ *   a's rows).  hits[j] = the number of points of a that are hits: an existence count, so no search order shows.
+ *   Search: each fragment is counting-sorted into a uniform cell grid over its finite rows (at most 2 rows + 64 cells;
+ *   edge 1.01 radius, grown by 1.25 until the cells fit; rows outside clamp into border cells).  A query p goes into
+ *   b's frame as q = R^T (p - t) (fp64) and scans every cell the box [q - r', q + r'] touches.  Margin: with delta =
+ *   max |(R^T R - I)_ik| (+ 2^-40), bmax = max |coordinate| of b's finite rows and B = max_i (sum_k |R_ik| bmax +
+ *   |t_i|) >= |b'_i|, a passing b' lies within D = radius (1 + 2^-20) of p (the fp32 d2 is at most 5 roundings below
+ *   the true square) and b' lies within 2^-23 B of R b + t (one fp32 rounding per coordinate, sqrt(3) 2^-24 B in norm,
+ *   plus the fp64 map's error); so |q - b| <= (D + 2^-23 B)(1 + 2 delta) + 6 delta bmax (|R^T w| <= ||R|| |w| and
+ *   ||R^T R - I||_F <= 3 delta), and r' adds 2^-40 (|p|_inf + |t|_inf + bmax) for q's own fp64 error.  The bound holds
+ *   for any R (a far-from-rigid R only widens the search); a non-finite r' or q scans every cell.
+ *   Refused before any launch: a job naming a fragment out of range, a fragment with no rows or more than
+ *   USIP_OVERLAP_MAX_ROWS, more than 65535 fragments, radius <= 0 or non-finite, scratch smaller than
+ *   usip_fragment_overlap_scratch_bytes(offsets[n_frags], n_frags, J) or not 16-byte aligned.  Six kernels per call:
+ *   box, grid set-up, count, scan, scatter, query. */
+#define USIP_OVERLAP_MAX_ROWS (1 << 26)
+size_t usip_fragment_overlap_scratch_bytes(int64_t total_rows, int n_frags, int J);
+int usip_fragment_overlap_f32(const float* xyz, const int64_t* offsets, int n_frags, const int32_t* jobs,
+                              const double* Rt, int J, float radius, void* scratch, size_t scratch_bytes,
+                              int32_t* hits, void* stream);
+
 /* Radius non-maximum suppression of the detected keypoints    evaluation/save_keypoints.py:180-216 (nms)
  * keypoints (B,3,M) f32, sigmas (B,M) f32 -> out_idx (B,M) i32: original indices of the kept keypoints in the order the
  * reference emits them (ascending sigma, ties by index), padded with -1; out_count (B,) i32.  radius < 0.01: pass-through

@@ -86,6 +86,11 @@ SIGNATURES = {
                                    c_int, ctypes.c_double, ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                    c_ptr]),
     "usip_ransac_uniforms": (c_int, [ctypes.c_uint64, c_int, c_ptr, c_ptr]),
+    "usip_ransac_info_f64": (c_int, [c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_ptr,
+                                     c_int, ctypes.c_double, ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr]),
+    "usip_fragment_overlap_scratch_bytes": (ctypes.c_size_t, [c_i64, c_int, c_int]),
+    "usip_fragment_overlap_f32": (c_int, [c_ptr, c_ptr, c_int, c_ptr, c_ptr, c_int, c_f32, c_ptr, ctypes.c_size_t, c_ptr,
+                                          c_ptr]),
     "usip_nms_f32":(c_int, [c_ptr, c_ptr, ctypes.c_float, c_ptr, c_ptr, c_int, c_int, c_ptr]),
     "usip_l2norm_bwd": (c_int, [c_ptr, c_ptr, c_int, c_ptr, c_int, c_int, c_int, c_int, c_ptr]),
     "usip_desc_triplet_bwd": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, ctypes.c_float, ctypes.c_float,
@@ -168,7 +173,7 @@ def load():
 WEIGHT_GEN = [0]
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
-KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_cloud_subsample": 2}
+KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_cloud_subsample": 2, "usip_fragment_overlap_f32": 6}
 LAUNCHES = [0]
 
 

@@ -49,6 +49,15 @@ __device__ __forceinline__ float sqdist_rn(float ax, float ay, float az, float b
   return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
 }
 
+// ((m0*x + m1*y) + m2*z) + m3 for the three rows of a row-major 3x4 map, fp64 without contraction (repeatability.cu's
+// order); registration.cu and overlap.cu map points with it.
+__device__ __forceinline__ void reg_map(const double* T, double& x, double& y, double& z) {
+  const double a = x, b = y, c = z;
+  x = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], a), __dmul_rn(T[1], b)), __dmul_rn(T[2], c)), T[3]);
+  y = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], a), __dmul_rn(T[5], b)), __dmul_rn(T[6], c)), T[7]);
+  z = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], a), __dmul_rn(T[9], b)), __dmul_rn(T[10], c)), T[11]);
+}
+
 // Philox4x32-10 (Salmon et al., SC'11): counter c, key (k0, k1) -> four random words.  pairgen.cu and registration.cu
 // build their counters from it.
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {

@@ -286,14 +286,6 @@ __device__ __forceinline__ bool reg_inlier(const double* Rt, double ax, double a
   return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz))) < thr;
 }
 
-// ((m0*x + m1*y) + m2*z) + m3 for the three rows of a row-major 3x4 map (repeatability.cu's order)
-__device__ __forceinline__ void reg_map(const double* T, double& x, double& y, double& z) {
-  const double a = x, b = y, c = z;
-  x = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], a), __dmul_rn(T[1], b)), __dmul_rn(T[2], c)), T[3]);
-  y = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], a), __dmul_rn(T[5], b)), __dmul_rn(T[6], c)), T[7]);
-  z = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], a), __dmul_rn(T[9], b)), __dmul_rn(T[10], c)), T[11]);
-}
-
 struct RegShared {                          // the static part of the RANSAC kernel's shared memory
   int32_t cnt[REG_THREADS];
   double Rt[12];
@@ -498,6 +490,118 @@ ransac_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ count, 
   }
 }
 
+// Column k of register2Fragments.m's A = [I3 | [[0, 2z, -2y], [-2z, 0, 2x], [2y, -2x, 0]]] at (x, y, z)
+__device__ __forceinline__ void reg_info_col(int k, double x, double y, double z, double a[3]) {
+  const double x2 = __dmul_rn(2.0, x), y2 = __dmul_rn(2.0, y), z2 = __dmul_rn(2.0, z);
+  a[0] = k == 0 ? 1.0 : k == 4 ? z2 : k == 5 ? -y2 : 0.0;
+  a[1] = k == 1 ? 1.0 : k == 3 ? -z2 : k == 5 ? x2 : 0.0;
+  a[2] = k == 2 ? 1.0 : k == 3 ? y2 : k == 4 ? -x2 : 0.0;
+}
+
+// one CTA per (pair, K): the information matrix of every trial budget's best model, from usip_ransac_rt_f64's
+// best_trial / status; dynamic smem: the points and match list of ransac_kernel, and the inlier flags
+__global__ void __launch_bounds__(REG_THREADS)
+ransac_info_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ count, int L,
+                   const int32_t* __restrict__ pairs, const double* __restrict__ frames, int nK,
+                   const int32_t* __restrict__ matches, const int32_t* __restrict__ n_matches, int cap, int nT,
+                   int tmax, double thr, uint64_t seed, const double* __restrict__ uni,
+                   const int32_t* __restrict__ best_in, const int32_t* __restrict__ status_in,
+                   double* __restrict__ info_out, int32_t* __restrict__ n_info_out) {
+  extern __shared__ __align__(16) double reg_smem[];
+  __shared__ double sRt[12];
+  __shared__ int32_t s_bad;
+  double* ax = reg_smem;
+  double* ay = ax + L;
+  double* az = ay + L;
+  double* px = az + L;
+  double* py = px + L;
+  double* pz = py + L;
+  uint32_t* mi = (uint32_t*)(pz + L);
+  uint8_t* flag = (uint8_t*)(mi + cap);
+  const int pk = blockIdx.x, p = pk / nK, tid = threadIdx.x;
+  const int sa = pairs[2 * p], sp = pairs[2 * p + 1];
+  const int na = min(count[sa], L), np = min(count[sp], L);
+  const int npts = min(max(n_matches[pk], 0), cap);
+  const double* F = frames + (int64_t)p * 36;
+  const int64_t ob = (int64_t)pk * nT;
+
+  if (tid == 0) s_bad = 0;
+  for (int i = tid; i < na; i += blockDim.x) {
+    const float* q = xyz + ((int64_t)sa * L + i) * 3;
+    double x = q[0], y = q[1], z = q[2];
+    reg_map(F, x, y, z);
+    ax[i] = x; ay[i] = y; az[i] = z;
+  }
+  for (int i = tid; i < np; i += blockDim.x) {
+    const float* q = xyz + ((int64_t)sp * L + i) * 3;
+    double x = q[0], y = q[1], z = q[2];
+    reg_map(F + 12, x, y, z);
+    px[i] = x; py[i] = y; pz[i] = z;
+  }
+  __syncthreads();
+  for (int m = tid; m < npts; m += blockDim.x) {
+    const int a = matches[((int64_t)pk * cap + m) * 2], b = matches[((int64_t)pk * cap + m) * 2 + 1];
+    if (a < 0 || a >= na || b < 0 || b >= np) { s_bad = 1; mi[m] = 0; }
+    else mi[m] = (uint32_t)a | ((uint32_t)b << 16);
+  }
+  __syncthreads();
+
+  for (int T = 0; T < nT; ++T) {
+    const int64_t o = ob + T;
+    const int b = best_in[o];
+    // register2Fragments.m's catch (status != 0): no inliers.  A status-0 entry that does not fit these matches (a
+    // best trial outside the stream, fewer than 3 matches) gives n_info -1.
+    const bool model = status_in[o] == 0;
+    const bool fits = !s_bad && (npts == 3 || (npts > 3 && b >= 0 && b <= tmax));
+    if (!model || !fits) {
+      if (tid < 36) info_out[o * 36 + tid] = 0.0;
+      if (tid == 0) n_info_out[o] = model ? -1 : 0;
+      continue;
+    }
+    if (npts == 3) {
+      for (int m = tid; m < 3; m += blockDim.x) flag[m] = 1;
+    } else {
+      if (tid == 0) {
+        double u[3]; int idx[3]; double x[3][3], y[3][3];
+        reg_uniforms(uni, b, seed, u);
+        reg_pick3(u, npts, idx);
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+          const uint32_t w = mi[idx[s]];
+          const int a = w & 0xffff, c = w >> 16;
+          x[s][0] = ax[a]; x[s][1] = ay[a]; x[s][2] = az[a];
+          y[s][0] = px[c]; y[s][1] = py[c]; y[s][2] = pz[c];
+        }
+        reg_fit3(x, y, sRt);
+      }
+      __syncthreads();
+      for (int m = tid; m < npts; m += blockDim.x) {
+        const uint32_t w = mi[m];
+        const int a = w & 0xffff, c = w >> 16;
+        flag[m] = reg_inlier(sRt, ax[a], ay[a], az[a], px[c], py[c], pz[c], thr);
+      }
+    }
+    __syncthreads();
+    if (tid < 36) {                                     // entry (r, c), summed over the inliers in match order
+      const int r = tid / 6, c = tid % 6;
+      double s = 0.0;
+      int n = 0;
+      for (int m = 0; m < npts; ++m) {
+        if (!flag[m]) continue;
+        const int a = mi[m] & 0xffff;
+        double ar[3], ac[3];
+        reg_info_col(r, ax[a], ay[a], az[a], ar);
+        reg_info_col(c, ax[a], ay[a], az[a], ac);
+        s = __dadd_rn(s, __dadd_rn(__dadd_rn(__dmul_rn(ar[0], ac[0]), __dmul_rn(ar[1], ac[1])), __dmul_rn(ar[2], ac[2])));
+        ++n;
+      }
+      info_out[o * 36 + tid] = s;
+      if (tid == 0) n_info_out[o] = n;
+    }
+    __syncthreads();
+  }
+}
+
 __global__ void ransac_uniforms_kernel(uint64_t seed, int T, double* __restrict__ out) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= T) return;
@@ -563,6 +667,30 @@ extern "C" int usip_ransac_rt_f64(const float* xyz, const int32_t* count, int n_
                                                                      n_matches, cap, t, nT, threshold, seed, uniforms,
                                                                      Rt, n_inliers, trialcount, best_trial, status);
   return check_launch("ransac_kernel");
+}
+
+extern "C" int usip_ransac_info_f64(const float* xyz, const int32_t* count, int n_scans, int L, const int32_t* pairs,
+                                    const double* frames, int P, int nK, const int32_t* matches,
+                                    const int32_t* n_matches, int cap, const int32_t* trials, int nT, double threshold,
+                                    uint64_t seed, const double* uniforms, const int32_t* best_trial,
+                                    const int32_t* status, double* info, int32_t* n_info, void* stream) {
+  USIP_REQUIRE(xyz && count && pairs && frames && matches && n_matches && trials && best_trial && status && info &&
+               n_info, "ransac_info: null pointer");
+  USIP_REQUIRE(n_scans > 0 && L > 0 && P > 0 && nK >= 1 && nK <= USIP_REP_MAX_K && cap >= 1, "ransac_info: bad sizes");
+  USIP_REQUIRE(L <= USIP_REG_MAX_KEYPOINTS, "ransac_info: more keypoints per scan than shared memory holds");
+  USIP_REQUIRE(cap <= 2 * USIP_REG_MAX_MATCH_K * L, "ransac_info: match list longer than 2 * 8 * L");
+  USIP_REQUIRE(nT >= 1 && nT <= USIP_REG_MAX_SWEEP, "ransac_info: 1 to USIP_REG_MAX_SWEEP trial budgets");
+  for (int i = 0; i < nT; ++i)
+    USIP_REQUIRE(trials[i] >= 1 && trials[i] <= USIP_REG_MAX_TRIALS && (i == 0 || trials[i] > trials[i - 1]),
+                 "ransac_info: trial budgets must ascend, be >= 1 and <= USIP_REG_MAX_TRIALS");
+  USIP_REQUIRE(threshold > 0.0, "ransac_info: the inlier threshold must be > 0");
+  const int smem = 6 * L * (int)sizeof(double) + cap * (int)sizeof(uint32_t) + ((cap + 15) / 16) * 16;
+  cudaError_t e = cudaFuncSetAttribute(ransac_info_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) { set_last_error("ransac_info: smem attribute"); return (int)e; }
+  ransac_info_kernel<<<P * nK, REG_THREADS, smem, (cudaStream_t)stream>>>(
+      xyz, count, L, pairs, frames, nK, matches, n_matches, cap, nT, trials[nT - 1], threshold, seed, uniforms,
+      best_trial, status, info, n_info);
+  return check_launch("ransac_info_kernel");
 }
 
 extern "C" int usip_ransac_uniforms(uint64_t seed, int T, double* out, void* stream) {

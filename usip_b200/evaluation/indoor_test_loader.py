@@ -105,6 +105,25 @@ def write_gt_log(path, entries):
             f.write("".join(" ".join("%.12e" % v for v in row) + "\n" for row in np.asarray(T).reshape(4, 4)))
 
 
+def write_gt_info(path, entries):
+    """A gt.info (mrWriteInfo.m's layout): per entry `anc pos count` and the 6x6, row by row."""
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    with open(path, "w") as f:
+        for anc, pos, count, M in entries:
+            f.write("%d\t%d\t%d\n" % (anc, pos, count))
+            f.write("".join(" ".join("%.12e" % v for v in row) + "\n" for row in np.asarray(M).reshape(6, 6)))
+
+
+def info_matrix(points):
+    """getGtInfoLog.m's covariance of correspondences q: sum over the points of G^T G, G = [I3, -[q]_x] -> (6, 6)."""
+    q = np.asarray(points, dtype=np.float64).reshape(-1, 3)
+    M = np.zeros((6, 6))
+    for x, y, z in q:
+        G = np.array([[1, 0, 0, 0, z, -y], [0, 1, 0, -z, 0, x], [0, 0, 1, y, -x, 0]], dtype=np.float64)
+        M += G.T @ G
+    return M
+
+
 def _gt_entries(rng, pairs, count):
     from .kitti_test_loader import random_rigid
     from .repeatability import gt_transform
@@ -120,15 +139,21 @@ def _gt_entries(rng, pairs, count):
 def write_synthetic_redwood(npy_root, gt_root, rows, pairs, seed=0, scenes=REDWOOD_SCENES):
     """A Redwood-shaped tree for tests and benchmarks: <npy_root>/<scene>/%d.npy, rows(scene index, frame) rows of
     synthetic_fragment each (rows may also be an int), and <gt_root>/original/<scene>-evaluation/gt.log listing
-    pairs[scene] [(anc, pos)] with random rigid transforms (the identity when anc == pos)."""
+    pairs[scene] [(anc, pos)] with random rigid transforms (the identity when anc == pos), and next to it a gt.info with
+    one info_matrix of 64 random room points per entry (drawn from their own stream, so the gt.log transforms do not
+    depend on it)."""
     rng = np.random.RandomState(seed)
+    info_rng = np.random.RandomState(seed + 7)
     for s, (scene, n) in enumerate(scenes):
         os.makedirs(os.path.join(npy_root, scene), exist_ok=True)
         for f in range(n):
             k = rows if np.isscalar(rows) else rows(s, f)
             np.save(os.path.join(npy_root, scene, "%d.npy" % f), synthetic_fragment(seed + 1000 * s + f, k))
-        write_gt_log(os.path.join(gt_root, "original", "%s-evaluation" % scene, "gt.log"),
-                     _gt_entries(rng, pairs.get(scene, []), n))
+        entries = _gt_entries(rng, pairs.get(scene, []), n)
+        evaluation = os.path.join(gt_root, "original", "%s-evaluation" % scene)
+        write_gt_log(os.path.join(evaluation, "gt.log"), entries)
+        write_gt_info(os.path.join(evaluation, "gt.info"),
+                      [(a, p, c, info_matrix(info_rng.uniform(-2, 2, (64, 3)))) for a, p, c, _ in entries])
 
 
 def write_synthetic_3dmatch(root, frames, rows, pairs, seed=0):

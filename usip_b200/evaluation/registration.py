@@ -274,8 +274,16 @@ class Registration:
 
 
 def descriptor_opt(dataset, **over):
-    """The reference's KITTI / Oxford descriptor options (kitti/options_descriptor.py, oxford/options_descriptor.py):
-    the detector's options plus ball_radius 2, ball_nsamples 64, descriptor_len 128, surface_normal_len 4."""
+    """The reference's descriptor options: KITTI / Oxford (kitti/ and oxford/options_descriptor.py) the detector's
+    options plus ball_radius 2, ball_nsamples 64, descriptor_len 128, surface_normal_len 4; Redwood and 3DMatch
+    (scenenn/options_descriptor.py) ball_radius 0.75, ball_nsamples 448, descriptor_len 128, sigma_max 0.5.  The
+    descriptor plan has no 448-sample ball group: those descriptors are scored from the reference's result tree
+    (read_descriptor_tree), or ball_nsamples is overridden."""
+    if dataset in ("redwood", "3dmatch"):
+        o = detector_opt(dataset, ball_radius=0.75, ball_nsamples=448, descriptor_len=128, surface_normal_len=4,
+                         sigma_max=0.5, triple_loss_gamma=0.3)
+        o.__dict__.update(over)
+        return o
     o = detector_opt(dataset, ball_radius=2.0, ball_nsamples=64, descriptor_len=128, surface_normal_len=4,
                      sigma_max=3.0, triple_loss_gamma=0.5)
     o.__dict__.update(over)

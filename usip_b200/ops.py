@@ -3,6 +3,7 @@ memory and streams only; every computation below happens in libusip_b200.so.  Al
 torch's current CUDA stream and never synchronise."""
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -371,6 +372,66 @@ def ransac_rt(xyz, count, pairs, frames, matches, n_matches, trials, threshold=1
             float(threshold), int(seed) & (2 ** 64 - 1), _p(uniforms), _p(Rt), _p(out["n_inliers"]),
             _p(out["trialcount"]), _p(out["best_trial"]), _p(out["status"]), _stream()), "usip_ransac_rt_f64")
     return out
+
+
+def ransac_info(xyz, count, pairs, frames, matches, n_matches, trials, best_trial, status, threshold=1.0, seed=0,
+                uniforms=None):
+    """register2Fragments.m's information matrix of ransac_rt's best models (include/usip_b200.h usip_ransac_info_f64):
+    the arguments of ransac_rt, plus its best_trial and status (P,nK,nT) i32 CUDA -> (info (P,nK,nT,6,6) f64, n_info
+    (P,nK,nT) i32)."""
+    _req(xyz, f32, "xyz"); _req(count, i32, "count"); _req(pairs, i32, "pairs"); _req(frames, torch.float64, "frames")
+    _req(matches, i32, "matches"); _req(n_matches, i32, "n_matches")
+    _req(best_trial, i32, "best_trial"); _req(status, i32, "status")
+    S, L, _ = xyz.shape
+    P, nK, cap = matches.shape[0], matches.shape[1], matches.shape[2]
+    trials = [int(t) for t in trials]
+    nT, dev = len(trials), xyz.device
+    if tuple(xyz.shape) != (S, L, 3) or tuple(count.shape) != (S,) or tuple(pairs.shape) != (P, 2):
+        raise ValueError("xyz must be (S, L, 3), count (S,) and pairs (P, 2)")
+    if tuple(frames.shape) != (P, 3, 3, 4) or tuple(matches.shape) != (P, nK, cap, 2) or \
+            tuple(n_matches.shape) != (P, nK):
+        raise ValueError("frames must be (P, 3, 3, 4), matches (P, nK, cap, 2) and n_matches (P, nK)")
+    if tuple(best_trial.shape) != (P, nK, nT) or tuple(status.shape) != (P, nK, nT):
+        raise ValueError("best_trial and status must be (P, nK, nT)")
+    if uniforms is not None:
+        _req(uniforms, torch.float64, "uniforms")
+        if not trials or tuple(uniforms.shape) != (max(trials) + 1, 3):
+            raise ValueError("uniforms must be (max(trials) + 1, 3)")
+    t_h = (ctypes.c_int32 * nT)(*trials)
+    info = torch.empty((P, nK, nT, 6, 6), dtype=torch.float64, device=dev)
+    n_info = torch.empty((P, nK, nT), dtype=i32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_ransac_info_f64(
+            _p(xyz), _p(count), S, L, _p(pairs), _p(frames), P, nK, _p(matches), _p(n_matches), cap, t_h, nT,
+            float(threshold), int(seed) & (2 ** 64 - 1), _p(uniforms), _p(best_trial), _p(status), _p(info),
+            _p(n_info), _stream()), "usip_ransac_info_f64")
+    return info, n_info
+
+
+def fragment_overlap(xyz, offsets, jobs, Rt, radius=0.2):
+    """register2Fragments.m's aligned-point count (include/usip_b200.h usip_fragment_overlap_f32): xyz (R,3) f32 CUDA,
+    every fragment's rows packed; offsets (n_frags + 1,) ints and jobs (J, 2) ints (fragment a, fragment b), host
+    (numpy or lists); Rt (J,3,4) f64 CUDA mapping b into a's frame -> hits (J,) i32 CUDA, the number of points of a
+    within `radius` of some mapped point of b."""
+    _req(xyz, f32, "xyz"); _req(Rt, torch.float64, "Rt")
+    offsets = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+    jobs = np.ascontiguousarray(jobs, dtype=np.int32).reshape(-1, 2)
+    nf, J = len(offsets) - 1, len(jobs)
+    if xyz.dim() != 2 or xyz.shape[1] != 3 or nf < 1 or int(offsets[-1]) != xyz.shape[0]:
+        raise ValueError("xyz must be (offsets[-1], 3) with at least one fragment")
+    if tuple(Rt.shape) != (J, 3, 4):
+        raise ValueError("Rt must be (J, 3, 4)")
+    hits = torch.empty((J,), dtype=i32, device=xyz.device)
+    if J == 0:
+        return hits
+    lib = _lib.load()
+    nbytes = int(lib.usip_fragment_overlap_scratch_bytes(int(offsets[-1]), nf, J))
+    scratch = torch.empty(((nbytes + 15) // 16, 4), dtype=i32, device=xyz.device)
+    with torch.cuda.device(xyz.device):
+        check(lib.usip_fragment_overlap_f32(_p(xyz), offsets.ctypes.data, nf, jobs.ctypes.data, _p(Rt), J,
+                                            float(radius), _p(scratch), nbytes, _p(hits), _stream()),
+              "usip_fragment_overlap_f32")
+    return hits
 
 
 def ransac_uniforms(T, seed=0, device="cuda"):
