@@ -47,9 +47,10 @@ int main(){ printf("%zu %zu %zu %zu %zu %zu\n", sizeof(usip_layer_desc), offseto
                    LayerDesc.gmax.offset, LayerDesc.precision.offset]
 
 
-def _misaligned_backward_calls():
-    """One call per (entry point, float4 operand) of the backward kernels with that operand 4 bytes off a 16-byte
-    boundary; every other pointer is aligned.  The addresses are never dereferenced: the argument check runs first."""
+def _misaligned_calls():
+    """One call per (entry point, float4 operand) of the backward kernels, segmax and knn_combine with that operand 4
+    bytes off a 16-byte boundary; every other pointer is aligned.  The addresses are never dereferenced: the argument
+    check runs first."""
     from usip_b200 import _lib
     lib = _lib.load()
     A = 0x100000
@@ -84,12 +85,21 @@ def _misaligned_backward_calls():
     aligned = ctypes.c_void_p(A + 0x40000)
     calls.append(("knn_combine_bwd", 0, lambda GY=GY: lib.usip_knn_combine_bwd(GY, 128, aligned, aligned, aligned, 128, aligned,
                                                                                 128, 1, 32, 16, 128, None)))
+    # forward kernels with float4 / int4 operands
+    for bad in range(3):      # X, pooled, arg
+        X, pooled, arg = ptrs(3, bad)
+        calls.append(("segmax", bad, lambda X=X, pooled=pooled, arg=arg:
+                      lib.usip_segmax(X, 64, aligned, aligned, pooled, 64, arg, 2, 500, 8, 64, None)))
+    for bad in range(2):      # Z, Y
+        Z, Y = ptrs(2, bad)
+        calls.append(("knn_combine", bad, lambda Z=Z, Y=Y:
+                      lib.usip_knn_combine(Z, 128, aligned, aligned, aligned, 128, aligned, Y, 128, aligned, 1, 32, 16, 128, None)))
     return lib, calls
 
 
 def test_backward_entry_points_reject_misaligned_operands():
     """A misaligned float4 operand is refused on the host (-1, no launch) -- it used to reach a kernel and fault the device."""
-    lib, calls = _misaligned_backward_calls()
+    lib, calls = _misaligned_calls()
     for name, bad, fn in calls:
         assert fn() == -1, (name, bad)
         assert b"aligned" in lib.usip_last_error(), (name, bad, lib.usip_last_error())

@@ -385,6 +385,8 @@ def test_head_finalize_and_bwd():
     out4 = randn(B * M, ld, g=g, scale=4.0)
     out4[0, 3], out4[1, 3], out4[2, 3], out4[3, 3] = 25.0, -50.0, 20.0, 19.5
     out4[4:20, 3] = torch.linspace(0.5, 19.0, 16, device=dev())         # (0, 20]: sigmoid, not the x > 20 shortcut
+    out4[20, 3] = float(np.nextafter(np.float32(20), np.float32(21)))   # the first value above the softplus threshold
+    out4[21, 3] = -100.0                                                # expf underflows to a subnormal
     cmean = randn(B, 3, M, g=g)
     kp, sig = torch.empty(B, 3, M, device=dev()), torch.empty(B, M, device=dev())
     call("usip_head_finalize", P(out4), ld, P(cmean), 0.001, P(kp), P(sig), B, M)

@@ -176,14 +176,17 @@ def test_som_assign_sort_mean_segmax():
 
 
 def test_knn_nodes_vs_oracle():
+    """Register kernel (M <= 512, K <= M) and shared-memory kernel (M > 512 up to its 3200-node limit, or K > M, whose
+    columns from M on are written as 0)."""
     from usip_b200 import ops
     rng = np.random.default_rng(4)
-    pts = rng.uniform(-10, 10, (4, 3, 200)).astype(np.float32)
-    pts[0, :, 50] = pts[0, :, 20]          # duplicate point -> exact ties
-    for K in (16, 32):
+    for B, M, K in ((4, 200, 16), (4, 200, 32), (2, 20, 8), (2, 512, 16), (2, 513, 16), (1, 3200, 32), (2, 20, 24)):
+        pts = rng.uniform(-10, 10, (B, 3, M)).astype(np.float32)
+        pts[0, :, M // 2] = pts[0, :, M // 5]          # duplicate point -> exact ties
         out = ops.knn_nodes(cu(pts), K).cpu().numpy()
-        ref, _ = orc.knn(pts, pts, K)
-        assert np.array_equal(out, ref)
+        ref, _ = orc.knn(pts, pts, min(K, M))
+        assert np.array_equal(out[:, :, :M], ref), (B, M, K)
+        assert np.all(out[:, :, M:] == 0), (B, M, K)
 
 
 def test_query_topk_api():
@@ -218,11 +221,15 @@ def _layer_ref(X, W, b, scale, shift, relu, addend, add_idx):
                                               # many tiles per CTA, ragged tails
                                               (16512, 256, 256, 16), (8320, 512, 512, 32), (16400, 64, 256, 0),
                                               # 128-wide column tiles with the cross-quarter group combine
-                                              (16896, 256, 256, 64)])
+                                              (16896, 256, 256, 64),
+                                              # the first-layer kernel at Cout = 32; SIMT groups of 4, 8 and 128 rows
+                                              (1000, 7, 32, 0), (4096, 64, 64, 4), (2048, 32, 64, 8), (4096, 128, 128, 128)])
 def test_layer_fwd(P, Cin, Cout, group, precision):
     from usip_b200 import ops
     if precision and not (Cin % 32 == 0 and Cout % 64 == 0):
         pytest.skip("tensor-core path needs Cin%32==0 and Cout%64==0")
+    if precision and group in (4, 8):
+        pytest.skip("tensor-core path takes groups of 16 to 128 rows")
     rng = np.random.default_rng(P + Cin)
     ldx = Cin + (8 - Cin % 8) % 8
     X = rng.normal(size=(P, ldx)).astype(np.float32)

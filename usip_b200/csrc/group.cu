@@ -414,7 +414,9 @@ index_max_smem_kernel(const float* __restrict__ data, const int32_t* __restrict_
   const int32_t* idx = index + (size_t)b * N;
   const float* base = data + ((size_t)b * C + c0) * N;
   const int nch = min(CPB, C - c0);
-  const bool vec_ok = (N % 4 == 0);
+  // int4 / float4 loads need every row start 16-byte aligned: N % 4 == 0 keeps the rows in step with the base pointers,
+  // which a view at an element offset (e.g. buf[1:]) does not align
+  const bool vec_ok = (N % 4 == 0) && ((reinterpret_cast<uintptr_t>(data) | reinterpret_cast<uintptr_t>(index)) & 15) == 0;
   if (vec_ok) {
     for (int n4 = tid; n4 * 4 < N; n4 += 256) {
       int4 k4 = *reinterpret_cast<const int4*>(idx + n4 * 4);
@@ -590,6 +592,9 @@ extern "C" int usip_cluster_mean_decenter(const float* xyz, const float* feat, c
 extern "C" int usip_segmax(const float* X, int ldx, const int32_t* seg_off, const int32_t* perm,
                            float* pooled, int ldp, int32_t* arg, int B, int N, int M, int C, void* stream) {
   USIP_REQUIRE(X && seg_off && perm && pooled && C % 4 == 0 && ldx % 4 == 0 && ldp % 4 == 0, "segmax: bad args");
+  // the kernel reads X and writes pooled as float4, arg as int4
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(pooled) | reinterpret_cast<uintptr_t>(arg)) & 15) == 0,
+               "segmax: X, pooled and arg must be 16-byte aligned");
   int warps = B * M;
   segmax_kernel<<<cdiv(warps * 32, 256), 256, 0, (cudaStream_t)stream>>>(X, ldx, seg_off, perm, pooled, ldp, arg,
                                                                        B, N, M, C);

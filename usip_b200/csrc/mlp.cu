@@ -656,6 +656,9 @@ extern "C" int usip_knn_combine(const float* Z, int ldz, const float* pts, const
                                 int ldw, const float* bias, float* Y, int ldy, float* stat_partial, int B, int M,
                                 int K, int Cout, void* stream) {
   USIP_REQUIRE(Z && pts && knn_idx && W && Y && Cout % 4 == 0 && ldz % 4 == 0 && ldy % 4 == 0, "knn_combine: bad args");
+  // the kernel reads Z and writes Y as float4
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(Z) | reinterpret_cast<uintptr_t>(Y)) & 15) == 0,
+               "knn_combine: Z and Y must be 16-byte aligned");
   size_t smem = (size_t)2 * 8 * Cout * sizeof(float);
   USIP_REQUIRE(smem <= 48 * 1024, "knn_combine: Cout too large");
   int G = B * M * K;
