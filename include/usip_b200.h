@@ -64,14 +64,17 @@ int usip_ball_group_scratch_init(void* scratch, int64_t scratch_bytes, int B, vo
 /* k-nearest-POINT grouping of the ablation detector RPN_Detector_KNN      models/networks.py:556-565
  * (torch.norm + topk(k, largest=False, sorted=False) + gather + subtract the node), without the (B,M,N) matrix.
  * out_idx (B,M,K) i32: the K points nearest to each centre, EXACT, in ascending point index (the reference's order is
- * unspecified; ties at the K-th distance: lowest index first); out_group / out_rows as in usip_ball_group_f32.  K <= N. */
+ * unspecified; ties at the K-th distance: lowest index first); out_group / out_rows as in usip_ball_group_f32.  K <= N.
+ * A NaN or inf squared distance gets one key, larger than every finite one, so such points come last and tie among
+ * themselves lowest index first (torch.topk would put NaN after inf). */
 int usip_knn_group_f32(const float* xyz, const float* feat, const float* centers, int32_t* out_idx, float* out_group,
                        float* out_rows, int ld_rows, int B, int S, int N, int M, int K, void* stream);
 
 /* Farthest point sampling of the SOM nodes          data/kitti_detector_loader.py:68-83 (FarthestSampler.sample), :144-145
  * pts (B, Ns, 3) f32 row-major (the numpy subset the reference samples from), start (B,) i32 = index of the first node
  * (the reference draws it with np.random.randint) -> out_idx (B, k) i32 in selection order, out_nodes (B, 3, k) f32 (or
- * NULL).  Bit-identical to the numpy code: float64 running distances, first arg-max.  Ns <= 8192. */
+ * NULL).  Bit-identical to the numpy code: float64 running distances, first arg-max.  Ns <= 8192.  Points must be finite:
+ * np.minimum propagates a NaN distance, the kernel keeps the smaller value. */
 int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float* out_nodes, int B, int Ns, int k,
                  void* stream);
 
@@ -302,7 +305,8 @@ int usip_fragment_overlap_f32(const float* xyz, const int64_t* offsets, int n_fr
 /* Radius non-maximum suppression of the detected keypoints    evaluation/save_keypoints.py:180-216 (nms)
  * keypoints (B,3,M) f32, sigmas (B,M) f32 -> out_idx (B,M) i32: original indices of the kept keypoints in the order the
  * reference emits them (ascending sigma, ties by index), padded with -1; out_count (B,) i32.  radius < 0.01: pass-through
- * (0..M-1, count M) like the reference. */
+ * (0..M-1, count M) like the reference.  NaN sigmas come first, in index order among themselves (np.argmin returns the
+ * first NaN), and each suppresses its neighbours as usual.  M <= 8533 (6 * 4 * M bytes of shared memory). */
 int usip_nms_f32(const float* keypoints, const float* sigmas, float radius, int32_t* out_idx, int32_t* out_count,
                  int B, int M, void* stream);
 
@@ -331,7 +335,7 @@ int usip_som_assign_grid_f32(const float* xyz, const float* node, int32_t* min_i
  *   seg_off (B,M+1) i32 : rows [seg_off[m], seg_off[m+1]) of cloud b belong to node m
  *   perm    (B,N)   i32 : sorted position -> original point index n (ascending n inside a node)
  *   row_seg (B,N)   i32 : b*M + node id of each sorted row
- * scratch: B * ceil(N/256) * M i32. */
+ * scratch: B * ceil(N/256) * M i32.  M <= 50176; a larger M is refused before any launch. */
 int usip_cluster_sort(const int32_t* min_idx, int32_t* seg_off, int32_t* perm, int32_t* row_seg,
                       int32_t* scratch, int B, int N, int M, void* stream);
 

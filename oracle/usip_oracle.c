@@ -158,15 +158,17 @@ void orc_fps(const float* pts, int start, int32_t* out_idx, int Ns, int k) {
 }
 
 /* evaluation/save_keypoints.py:180-216 nms(): kp (M,3) row-major, float32 np.linalg.norm distances, kept while
- * distance > radius; the next keypoint is always the FIRST arg-min of sigma among the remaining ones.  Returns the
- * number of kept keypoints, their original indices in emission order in out_idx. */
+ * distance > radius; the next keypoint is always the FIRST arg-min of sigma among the remaining ones (np.argmin returns
+ * the first NaN when there is one, so NaN sigmas go first, in index order).  Returns the number of kept keypoints, their
+ * original indices in emission order in out_idx. */
 int orc_nms(const float* kp, const float* sigma, float radius, int32_t* out_idx, int M) {
   if (radius < 0.01f) { for (int i = 0; i < M; ++i) out_idx[i] = i; return M; }
   uint8_t* gone = (uint8_t*)calloc((size_t)M, 1);
   int count = 0;
   for (;;) {
     int best = -1;
-    for (int i = 0; i < M; ++i) if (!gone[i] && (best < 0 || sigma[i] < sigma[best])) best = i;
+    for (int i = 0; i < M; ++i)
+      if (!gone[i] && (best < 0 || (isnan(sigma[i]) && !isnan(sigma[best])) || sigma[i] < sigma[best])) best = i;
     if (best < 0) break;
     out_idx[count++] = best;
     for (int j = 0; j < M; ++j) {

@@ -105,6 +105,27 @@ def test_backward_entry_points_reject_misaligned_operands():
         assert b"aligned" in lib.usip_last_error(), (name, bad, lib.usip_last_error())
 
 
+def test_neighbour_entry_points_refuse_before_launch():
+    """Sizes the neighbour-search, sampling and NMS kernels cannot take are refused on the host (-1, no launch): the
+    addresses are never dereferenced, and a launch on a machine without a GPU would fail with a CUDA error instead."""
+    from usip_b200 import _lib
+    lib = _lib.load()
+    a = [ctypes.c_void_p(0x100000 + 0x10000 * i) for i in range(8)]
+    calls = [
+        ("nms M = 8534", lambda: lib.usip_nms_f32(a[0], a[1], 1.0, a[2], a[3], 1, 8534, None), b"M too large"),
+        ("fps Ns = 8193", lambda: lib.usip_fps_f32(a[0], a[1], a[2], a[3], 1, 8193, 16, None), b"8192"),
+        ("knn_group K > N", lambda: lib.usip_knn_group_f32(a[0], a[1], a[2], a[3], a[4], a[5], 8, 1, 4, 100, 16, 101, None),
+         b"K <= N"),
+        ("knn_group S = 6", lambda: lib.usip_knn_group_f32(a[0], a[1], a[2], a[3], a[4], a[5], 16, 1, 6, 100, 16, 8, None),
+         b"S <= 5"),
+        ("cluster_sort M too large", lambda: lib.usip_cluster_sort(a[0], a[1], a[2], a[3], a[4], 1, 1000, 50177, None),
+         b"M too large"),
+    ]
+    for name, fn, msg in calls:
+        assert fn() == -1, name
+        assert msg in lib.usip_last_error(), (name, lib.usip_last_error())
+
+
 def test_product_path_fails_loudly_without_cuda():
     import torch
     if torch.cuda.is_available():

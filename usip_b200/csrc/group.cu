@@ -555,6 +555,9 @@ extern "C" int usip_som_assign_f32(const float* xyz, const float* node, int32_t*
 extern "C" int usip_cluster_sort(const int32_t* min_idx, int32_t* seg_off, int32_t* perm, int32_t* row_seg,
                                  int32_t* scratch, int B, int N, int M, void* stream) {
   USIP_REQUIRE(min_idx && seg_off && perm && row_seg && scratch, "cluster_sort: bad args");
+  // the scan kernel holds M totals + 1024 partials in shared memory: refuse before the first launch
+  const size_t smem = (size_t)(M + 1024) * sizeof(int);
+  USIP_REQUIRE(smem <= 200 * 1024, "cluster_sort: M too large");
   cudaStream_t st = (cudaStream_t)stream;
   const int chunks = cdiv(N, SORT_CHUNK);
   dim3 grid(chunks, B);
@@ -569,8 +572,6 @@ extern "C" int usip_cluster_sort(const int32_t* min_idx, int32_t* seg_off, int32
   } else {
     sort_hist_kernel<<<grid, SORT_CHUNK, 0, st>>>(min_idx, scratch, N, M, chunks);
   }
-  size_t smem = (size_t)(M + 1024) * sizeof(int);
-  USIP_REQUIRE(smem <= 200 * 1024, "cluster_sort: M too large");
   if (smem > 48 * 1024) cudaFuncSetAttribute(sort_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   sort_scan_kernel<<<B, 1024, smem, st>>>(scratch, seg_off, N, M, chunks);
   if (match) sort_place_match_kernel<<<grid, SORT_CHUNK, msm, st>>>(min_idx, scratch, seg_off, perm, row_seg, N, M, chunks);

@@ -3,8 +3,8 @@
 //
 // Reference: evaluation/save_keypoints.py:180-216 nms(): repeat { take the remaining keypoint with the smallest sigma
 // (np.argmin: first minimum), emit it, drop every remaining keypoint whose float32 np.linalg.norm distance to it is not
-// > NMS_radius }.  Equivalent single sweep: visit the keypoints in (sigma, index) order and emit the ones no earlier
-// emitted keypoint has suppressed.  One CTA per cloud; the sweep is sequential in the keypoints, parallel in the
+// > NMS_radius }.  Equivalent single sweep: visit the keypoints in (sigma, index) order, NaN sigmas first, and emit the
+// ones no earlier emitted keypoint has suppressed.  One CTA per cloud; the sweep is sequential in the keypoints, parallel in the
 // suppression test.  Distances use the repository's fp32 policy (sqdist_rn + correctly rounded sqrt == numpy).
 #include "common.cuh"
 
@@ -34,11 +34,18 @@ nms_kernel(const float* __restrict__ kp, const float* __restrict__ sigma, float 
     if (tid == 0) out_count[b] = M;
     return;
   }
-  // rank by (sigma, index): the order in which repeated first-arg-min would visit the keypoints
+  // rank by (sigma, index): the order in which repeated first-arg-min would visit the keypoints.  np.argmin returns the
+  // first NaN when there is one, so NaN sigmas come before every finite one, in index order among themselves; the ranks
+  // are then a permutation of 0..M-1 and every order[] slot is written.
   for (int i = tid; i < M; i += NMS_THREADS) {
     const float si = ss[i];
+    const bool ni = si != si;
     int rk = 0;
-    for (int j = 0; j < M; ++j) { const float sj = ss[j]; rk += (sj < si || (sj == si && j < i)) ? 1 : 0; }
+    for (int j = 0; j < M; ++j) {
+      const float sj = ss[j];
+      const bool nj = sj != sj;
+      rk += (ni ? (nj && j < i) : (nj || sj < si || (sj == si && j < i))) ? 1 : 0;
+    }
     order[rk] = i;
   }
   __syncthreads();
