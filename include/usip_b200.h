@@ -133,7 +133,10 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  * usip_cloud_gather_candidates_zscaled: usip_cloud_gather_candidates with z multiplied by z_scale[c] (2*n_pairs) f32 in
  *   fp32, the height-scaled FPS input of the Oxford detector.
  * usip_scale_channel_f32: t (B, C, L) f32 in place, t[b, k, :] *= factor in fp32 (the descriptor batch's height
- *   scaling, oxford/train_descriptor.py). */
+ *   scaling, oxford/train_descriptor.py).
+ * Every cloud of the augment and gather calls is one grid row, so usip_pair_augment, usip_desc_pair_augment,
+ *   usip_modelnet_pair_augment and usip_cloud_gather_candidates(_zscaled) take n_pairs <= 32767 (-1 before any launch
+ *   above it); usip_test_cloud_gather takes n_clouds <= 65535 and usip_scale_channel_f32 B <= 65535. */
 #define USIP_PAIR_TRAIN 1
 #define USIP_PAIR_ROT_HORIZONTAL 2
 #define USIP_PAIR_ROT_3D 4

@@ -126,6 +126,31 @@ def test_neighbour_entry_points_refuse_before_launch():
         assert msg in lib.usip_last_error(), (name, lib.usip_last_error())
 
 
+@pytest.mark.parametrize("n_pairs", [32768, 40000])
+def test_pair_builders_refuse_more_pairs_than_grid_rows(n_pairs):
+    """Every cloud of the augment and gather kernels is one grid row (2 * n_pairs <= 65535): more pairs are refused on
+    the host (-1, no launch) instead of failing the launch or leaving clouds unwritten."""
+    from usip_b200 import _lib
+    lib = _lib.load()
+    a = [ctypes.c_void_p(0x100000 + 0x10000 * i) for i in range(10)]
+    outs9 = a[1:10]
+    calls = [
+        ("pair_augment", lambda: lib.usip_pair_augment(a[0], 8, a[0], a[0], a[0], a[0], a[0], None, None, None, 0, 0, 1,
+                                                       4, n_pairs, 16, 4, *outs9, None)),
+        ("modelnet_pair_augment", lambda: lib.usip_modelnet_pair_augment(
+            a[0], 6, a[0], a[0], a[0], a[0], a[0], None, None, None, 0, 0, 1, 3, n_pairs, 16, 4, *outs9, None)),
+        ("desc_pair_augment", lambda: lib.usip_desc_pair_augment(a[0], 8, a[0], a[0], a[0], a[0], a[0], None, None, None,
+                                                                 0, 0, 1, 4, n_pairs, 16, 4, *outs9[:6], None)),
+        ("cloud_gather_candidates", lambda: lib.usip_cloud_gather_candidates(a[0], 8, a[0], a[0], a[0], a[0], a[1],
+                                                                             n_pairs, 16, 5, None)),
+        ("cloud_gather_candidates", lambda: lib.usip_cloud_gather_candidates_zscaled(
+            a[0], 8, a[0], a[0], a[0], a[0], a[2], a[1], n_pairs, 16, 5, None)),
+    ]
+    for name, fn in calls:
+        assert fn() == -1, name
+        assert (name + ": at most 32767 pairs").encode() in lib.usip_last_error(), (name, lib.usip_last_error())
+
+
 def test_product_path_fails_loudly_without_cuda():
     import torch
     if torch.cuda.is_available():

@@ -26,6 +26,7 @@ constexpr int PG_AUG_THREADS = 256;
 constexpr uint32_t PG_SENTINEL = 0xffffffffu;      // key of a point that may not be drawn (outside the radius)
 constexpr int PG_PARAM_STRIDE = 48;                // doubles per pair, see usip_pair_augment in the header
 constexpr int PG_DESC_PARAM_STRIDE = 32;           // doubles per cloud, see usip_desc_pair_augment in the header
+constexpr int PG_MAX_PAIRS = 32767;                // 2*n_pairs clouds run in grid.y, at most 65535
 
 enum { PURPOSE_ROWS = 0, PURPOSE_CAND = 1, PURPOSE_START = 2, PURPOSE_JIT_PC = 3, PURPOSE_JIT_SN = 4,
        PURPOSE_JIT_NODE = 5, PURPOSE_NOISE = 6 };
@@ -785,6 +786,7 @@ static int pg_gather(const float* scans, int C, const int64_t* offsets, const in
                      int n_cand, void* stream) {
   USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && cand && out_pts, "cloud_gather_candidates: null pointer");
   USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N, "cloud_gather_candidates: bad sizes");
+  USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "cloud_gather_candidates: at most 32767 pairs");
   dim3 grid(cdiv(n_cand, 256), 2 * n_pairs);
   pair_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of_cloud, rows, cand, z_scale,
                                                               out_pts, N, n_cand);
@@ -841,6 +843,7 @@ extern "C" int usip_desc_pair_augment(const float* scans, int C, const int64_t* 
   USIP_REQUIRE(!(flags & USIP_PAIR_HEIGHT_SCALE), "desc_pair_augment: no height scaling in the descriptor's clouds");
   USIP_REQUIRE(!(flags & USIP_PAIR_ENU_TO_CAM) || S >= 3, "desc_pair_augment: the camera frame needs S >= 3");
   USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "desc_pair_augment: bad sizes");
+  USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "desc_pair_augment: at most 32767 pairs");
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
   desc_pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
       scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, N, M,
@@ -862,6 +865,7 @@ extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offse
   USIP_REQUIRE(!(flags & USIP_PAIR_HEIGHT_SCALE) || (flags & USIP_PAIR_ENU_TO_CAM),
                "pair_augment: height scaling is part of the ENU frame step");
   USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "pair_augment: bad sizes");
+  USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "pair_augment: at most 32767 pairs");
   const int sn_col = S == 1 ? C - 1 : 3;           // kitti_detector_loader.py:135-139
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
   pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
@@ -882,6 +886,7 @@ extern "C" int usip_modelnet_pair_augment(const float* scans, int C, const int64
                "modelnet_pair_augment: null output");
   USIP_REQUIRE(S == 3 && C >= 6, "modelnet_pair_augment: sn is columns 3:6 (S == 3, C >= 6)");
   USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "modelnet_pair_augment: bad sizes");
+  USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "modelnet_pair_augment: at most 32767 pairs");
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
   modelnet_pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
       scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, N, M, src_pc,
