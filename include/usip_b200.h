@@ -106,7 +106,8 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *   rows as above, nodes (2*n_pairs, 3, M) f32 = the FPS nodes (usip_fps_f32 out_nodes);
  *   params (n_pairs, 48) f64 per pair: [0:9] horizontal, [9:18] 3-d and [18:27] perturbation rotation matrices (row
  *     major, applied as data @ R in float64), [27] augmentation scale, [28:31] augmentation shift, [31:40] the transform's
- *     R (fp32 values), [40:43] its shift, [43] its scale, [44] the Oxford height scale (USIP_PAIR_HEIGHT_SCALE);
+ *     R (fp32 values), [40:43] its shift, [43] its scale, [44] the Oxford height scale (USIP_PAIR_HEIGHT_SCALE),
+ *     [45] the indoor per-pair augmentation switch (usip_indoor_pair_augment; ignored here), [46:48] unused;
  *   jit_pc (2*n_pairs, N, 3), jit_sn (2*n_pairs, N, S), jit_node (2*n_pairs, M, 3) f64 clipped jitter, each NULL to draw
  *     it on the device (N(0, 0.04^2) clipped at 0.12 for pc / node, N(0, 0.01^2) clipped at 0.05 for sn);
  *   flags: USIP_PAIR_* below.  sn = columns 3:3+S of the scan, or the last column when S == 1.
@@ -125,6 +126,15 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *     the pair, N(0, 0.01^2) clipped at 0.05 for pc and sn, N(0, 0.04^2) clipped at 0.1 for nodes;
  *   S == 3 and sn = columns 3:6 (C >= 6).  After any rotation sn is a float64 chain (rotated, jittered, times [27]);
  *     without one it is fp32, jittered and scaled in place.  sn is never shifted.  pc and nodes: as usip_pair_augment.
+ * usip_indoor_pair_augment (data/match3d_detector_loader.py:110-216 and scenenn_detector_loader.py, which augment like
+ *   KittiLoader with other laws, then transform_pc_pytorch for dst): arguments, params layout, arithmetic and outputs as
+ *   usip_pair_augment, but
+ *   - device-mode jitter is N(0, 0.01^2) clipped at 0.02 for pc, every sn column and nodes (same Philox keys);
+ *   - sn = columns 3:3+S for every S, 1 <= S <= 8 and 3 + S <= C;
+ *   - with USIP_PAIR_TRAIN, pair b is augmented only when params[b, 45] != 0 (SceneNN trains on its train split, which
+ *     is augmented, and its val split, which is not).  An un-augmented pair gets the gathered rows and nodes, then the
+ *     dst transform, exactly as in test mode; its jitter rows are never read;
+ *   - USIP_PAIR_ENU_TO_CAM and USIP_PAIR_HEIGHT_SCALE are refused (-1 before any launch).
  * Oxford scans (data/oxford_detector_loader.py, oxford_descriptor_loader.py) are ENU, z up.  USIP_PAIR_ENU_TO_CAM makes
  *   usip_pair_augment and usip_desc_pair_augment first map every row and node to the camera frame, (x, y, z) ->
  *   (x, -z, y), and sn columns 0:3 alike (requires S >= 3); then they run as above.  USIP_PAIR_HEIGHT_SCALE (detector
@@ -134,8 +144,8 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *   fp32, the height-scaled FPS input of the Oxford detector.
  * usip_scale_channel_f32: t (B, C, L) f32 in place, t[b, k, :] *= factor in fp32 (the descriptor batch's height
  *   scaling, oxford/train_descriptor.py).
- * Every cloud of the augment and gather calls is one grid row, so usip_pair_augment, usip_desc_pair_augment,
- *   usip_modelnet_pair_augment and usip_cloud_gather_candidates(_zscaled) take n_pairs <= 32767 (-1 before any launch
+ * Every cloud of the augment and gather calls is one grid row, so usip_pair_augment, usip_indoor_pair_augment,
+ *   usip_desc_pair_augment, usip_modelnet_pair_augment and usip_cloud_gather_candidates(_zscaled) take n_pairs <= 32767 (-1 before any launch
  *   above it); usip_test_cloud_gather takes n_clouds <= 65535 and usip_scale_channel_f32 B <= 65535. */
 #define USIP_PAIR_TRAIN 1
 #define USIP_PAIR_ROT_HORIZONTAL 2
@@ -162,6 +172,12 @@ int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const i
                       const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
                       int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node, float* dst_pc,
                       float* dst_sn, float* dst_node, float* R, float* scale, float* shift, void* stream);
+int usip_indoor_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                             const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
+                             const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags,
+                             int S, int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node,
+                             float* dst_pc, float* dst_sn, float* dst_node, float* R, float* scale, float* shift,
+                             void* stream);
 int usip_modelnet_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                                const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,
                                const double* jit_sn, const double* jit_node, uint64_t seed, uint64_t step, int flags,

@@ -1,15 +1,22 @@
-"""Cost of building detector training pairs (usip_b200.data.kitti_detector_loader, .modelnet_shrec_loader) -- one
-JSON line.
+"""Cost of building detector training pairs (usip_b200.data.kitti_detector_loader, .modelnet_shrec_loader,
+.match3d_detector_loader, .scenenn_detector_loader) -- one JSON line.
 
   * builder: ms per batch of B pairs in device mode (CUDA events), split into subsample / candidate gather + FPS /
     augment, and the augment kernel's GB/s against its compulsory bytes;
-  * reference: ms per pair of the reference's KittiLoader / ModelNet_Shrec_Loader.__getitem__ on the host cores (only
-    where the reference's Python tree is importable; otherwise "not measured");
-  * training loop: KittiPairSource / ModelNetPairSource + optimize() per step against optimize() on one resident batch.
+  * reference: ms per pair of the reference's KittiLoader / ModelNet_Shrec_Loader / Match3DDetectorLoader /
+    SceneNNDetectorLoader.__getitem__ on the host cores (only where the reference's Python tree is importable;
+    otherwise "not measured");
+  * training loop: KittiPairSource / ModelNetPairSource / Match3DPairSource / SceneNNPairSource ("train+val") +
+    optimize() per step against optimize() on one resident batch.
 
     python tools/bench_pairgen.py [--dataset kitti] [--pairs 8] [--scan-rows 20480] [--N 16384] [--M 512] [--out FILE]
     python tools/bench_pairgen.py --dataset modelnet    # defaults B=24, 10000-row objects, N=5000, M=512 (configs[1])
+    python tools/bench_pairgen.py --dataset 3dmatch     # B=2, N=10240, M=512, S=4 (match3d/options_detector.py)
+    python tools/bench_pairgen.py --dataset scenenn     # the same options, FPS over N/4
     python tools/bench_pairgen.py --reference-only      # host timing of the reference loader alone
+
+The indoor fragment sizes are assumptions, not measurements of the datasets: 250,000 rows for 3DMatch (about the size
+of its test fragments) and 30,000 for SceneNN.
 """
 import argparse
 import json
@@ -27,10 +34,15 @@ sys.path.insert(0, ROOT)
 
 from usip_b200 import ops  # noqa: E402
 from usip_b200.data import kitti_detector_loader as kdl  # noqa: E402
+from usip_b200.data import match3d_detector_loader as m3l  # noqa: E402
 from usip_b200.data import modelnet_shrec_loader as mnl  # noqa: E402
+from usip_b200.data import scenenn_detector_loader as snl  # noqa: E402
+from usip_b200.evaluation.indoor_test_loader import synthetic_fragment  # noqa: E402
 
 # per dataset: (pairs, scan rows, N, M), S, the builder, the source and the model's configuration
-DEFAULTS = {"kitti": (8, 20480, 16384, 512), "modelnet": (24, 10000, 5000, 512)}
+DEFAULTS = {"kitti": (8, 20480, 16384, 512), "modelnet": (24, 10000, 5000, 512), "3dmatch": (2, 250000, 10240, 512),
+            "scenenn": (2, 30000, 10240, 512)}
+INDOOR_DIVISOR = {"3dmatch": m3l.MATCH3D_DIVISOR, "scenenn": snl.SCENENN_DIVISOR}
 MN_SHAPES = ("airplane", "night_stand", "cup")
 
 
@@ -49,8 +61,22 @@ def modelnet_opt(N, M, B, device):
                     device=device)
 
 
+def indoor_opt(N, M, B, device):
+    """match3d/options_detector.py and scenenn/options_detector.py: rot_3d only, S=4, Kn=32."""
+    from tests.util_gpu import make_opt
+    return make_opt(input_pc_num=N, node_num=M, batch_size=B, surface_normal_len=4, node_knn_k_1=32, scene="indoor",
+                    loss_sigma_lower_bound=1e-4, keypoint_on_pc_alpha=10.0, rot_horizontal=False, rot_3d=True,
+                    rot_perturbation=False, translation_perturbation=False, device=device)
+
+
 def setup(a, dev):
     """-> (S, opt, builder class, scan generator, augment call(scans, off, sp, rows, nodes, params, flags))."""
+    if a.dataset in INDOOR_DIVISOR:
+        div = INDOOR_DIVISOR[a.dataset]
+        aug = lambda sc, off, sp, rows, nodes, params, flags: ops.indoor_pair_augment(sc, off, sp, rows, nodes, params,
+                                                                                      4, flags, 1, 0)
+        builder = lambda opt, mode, d, seed: m3l.IndoorPairBuilder(opt, mode, d, seed, divisor=div)
+        return 4, indoor_opt(a.N, a.M, a.pairs, dev), builder, synthetic_fragment, aug
     if a.dataset == "modelnet":
         aug = lambda *x: ops.modelnet_pair_augment(*x, 1, 0)
         return 3, modelnet_opt(a.N, a.M, a.pairs, dev), mnl.ModelNetPairBuilder, mnl.synthetic_object, aug
@@ -106,7 +132,15 @@ def bench_training_loop(a, dev):
     B, N, M = a.pairs, a.N, a.M
     S, opt, _, _, _ = setup(a, dev)
     with tempfile.TemporaryDirectory() as root:
-        if a.dataset == "modelnet":
+        if a.dataset == "3dmatch":
+            m3l.write_synthetic_3dmatch_train(root, {"train": {"scene": {"seq-01": B * a.loop_batches}}}, a.scan_rows,
+                                              seed=5)
+            src = m3l.Match3DPairSource(root, "train", opt, dev, seed=2)
+        elif a.dataset == "scenenn":                               # a quarter of the items are val items
+            n = B * a.loop_batches
+            snl.write_synthetic_scenenn(root, {"train": n - n // 4, "val": n // 4}, a.scan_rows, seed=5)
+            src = snl.SceneNNPairSource(root, "train+val", opt, dev, seed=2)
+        elif a.dataset == "modelnet":
             mnl.write_synthetic_modelnet(root, MN_SHAPES, -(-B * a.loop_batches // len(MN_SHAPES)), 0, a.scan_rows,
                                          seed=5)
             src = mnl.ModelNetPairSource(root, "train", opt, dev, seed=2)
@@ -114,7 +148,8 @@ def bench_training_loop(a, dev):
             kdl.write_synthetic_kitti(root, [B * a.loop_batches] + [0] * 10, a.scan_rows, seed=5)
             src = kdl.KittiPairSource(root, "train", opt, dev, seed=2)
         md = ModelDetector(opt)
-        load_params(md.detector, orc.init_detector_params(S=S, seed=1, randomize_bn=True))
+        C1, C2 = (64, 256) if opt.scene == "indoor" else (128, 512)       # keypoint_detector.py: the indoor widths
+        load_params(md.detector, orc.init_detector_params(S=S, seed=1, C1=C1, C2=C2, randomize_bn=True))
         for _ in range(2):                                        # warm-up: graph capture, allocator
             for _ in src.feed(md):
                 md.optimize(epoch=0)
@@ -140,21 +175,33 @@ def bench_training_loop(a, dev):
 
 
 def bench_reference(a):
-    """KittiLoader / ModelNet_Shrec_Loader.__getitem__ of the reference on the host, from a staged synthetic tree (N, M
-    as configured)."""
+    """KittiLoader / ModelNet_Shrec_Loader / Match3DDetectorLoader / SceneNNDetectorLoader.__getitem__ of the reference
+    on the host, from a staged synthetic tree (N, M as configured)."""
     modelnet = a.dataset == "modelnet"
+    module = {"modelnet": "data.modelnet_shrec_loader", "3dmatch": "data.match3d_detector_loader",
+              "scenenn": "data.scenenn_detector_loader"}.get(a.dataset, "data.kitti_detector_loader")
     try:
         import importlib
         from oracle import ref_shim
         if not ref_shim.reference_available():
             return None
         ref_shim.install(use_ref_ext=False)
-        kl = importlib.import_module("data.modelnet_shrec_loader" if modelnet else "data.kitti_detector_loader")
+        kl = importlib.import_module(module)
     except Exception as e:                                          # the reference tree is optional
         print("[bench_pairgen] reference loader not importable: %s" % e, file=sys.stderr)
         return None
     with tempfile.TemporaryDirectory() as root:
-        if modelnet:
+        if a.dataset in INDOOR_DIVISOR:
+            opt = ref_shim.make_opt(input_pc_num=a.N, node_num=a.M, surface_normal_len=4, rot_horizontal=False,
+                                    rot_3d=True, rot_perturbation=False, translation_perturbation=False)
+            if a.dataset == "3dmatch":
+                m3l.write_synthetic_3dmatch_train(root, {"train": {"scene": {"seq-01": a.ref_items}}}, a.scan_rows,
+                                                  seed=5)
+                loader = kl.Match3DDetectorLoader(root, "train", opt)
+            else:
+                snl.write_synthetic_scenenn(root, {"train": a.ref_items}, a.scan_rows, seed=5)
+                loader = kl.SceneNNDetectorLoader(root, "train", opt)
+        elif modelnet:
             opt = ref_shim.make_opt(dataset="modelnet", classes=40, input_pc_num=a.N, node_num=a.M,
                                     surface_normal_len=3, rot_horizontal=False, rot_3d=True, rot_perturbation=False,
                                     translation_perturbation=False)

@@ -465,6 +465,81 @@ def golden_modelnet_pairs(ref):
     print("modelnet_pairs.npz", os.path.getsize(os.path.join(OUT, "modelnet_pairs.npz")) // 1024, "KB")
 
 
+# data/match3d_detector_loader.py Match3DDetectorLoader.__getitem__ and data/scenenn_detector_loader.py
+# SceneNNDetectorLoader.__getitem__ on synthetic trees (usip_b200.data.match3d_detector_loader.write_synthetic_3dmatch_train,
+# scenenn_detector_loader.write_synthetic_scenenn), every fragment a (rows, 7) synthetic_fragment.  The 3DMatch
+# loader lists folders with os.listdir, so every item is recorded by its path relative to the tree's root.  One
+# SceneNN case runs a train item and then a val item from one seed: the mixed batch of scenenn/train_detector.py.
+IN_N, IN_M, IN_SEED = 1024, 64, 7500
+IN_M3_LAYOUT = {"train": {"kitchen": {"seq-01": 3, "seq-02": 2}, "office": {"seq-01": 2}},
+                "test": {"lab": {"seq-01": 2}}}
+IN_M3_ROWS = [1500, 1500, 700, 1500, 1500, 1500, 1500, 1500, 1500]      # file i in listing order; file 2 < N
+IN_M3_CASES = {     # name: (mode, relative paths, np seed, S, rot_horizontal, rot_3d, rot_perturbation, translation)
+    "m3_default": ("train", ["kitchen/seq-01/2.npy", "office/seq-01/0.npy"], 61, 4, 0, 1, 0, 0),   # options defaults
+    "m3_horizontal": ("train", ["kitchen/seq-02/1.npy"], 62, 4, 1, 0, 1, 1),
+    "m3_s3": ("train", ["kitchen/seq-01/0.npy"], 63, 3, 0, 1, 0, 0),
+    "m3_test": ("test", ["lab/seq-01/1.npy"], 64, 4, 0, 1, 0, 0),
+}
+IN_SN_COUNTS = {"train": 3, "val": 2, "test": 2}
+IN_SN_CASES = {     # name: ([(split, item)], np seed); scenenn/options_detector.py defaults (S 4, rot_3d)
+    "sn_train": ([("train", 1)], 71),                  # train item 1 has fewer than N rows
+    "sn_val": ([("val", 0)], 72),
+    "sn_test": ([("test", 1)], 73),
+    "sn_mixed": ([("train", 2), ("val", 1)], 74),
+}
+
+
+def indoor_scenenn_rows(split, i):
+    return 600 if (split, i) == ("train", 1) else 1300
+
+
+def golden_indoor_pairs(ref):
+    import importlib
+    import tempfile
+    from usip_b200.data.match3d_detector_loader import write_synthetic_3dmatch_train
+    from usip_b200.data.scenenn_detector_loader import write_synthetic_scenenn
+    m3 = importlib.import_module("data.match3d_detector_loader")
+    sn = importlib.import_module("data.scenenn_detector_loader")
+    keys = ("src_pc", "src_sn", "src_node", "dst_pc", "dst_sn", "dst_node", "R", "scale", "shift")
+    out = {"N": np.int64(IN_N), "M": np.int64(IN_M), "tree/seed": np.int64(IN_SEED),
+           "m3/layout": np.array(["%s/%s/%s/%d" % (split, scene, sub, n) for split, scenes in IN_M3_LAYOUT.items()
+                                  for scene, subs in scenes.items() for sub, n in subs.items()]),
+           "m3/rows": np.array(IN_M3_ROWS, dtype=np.int64),
+           "sn/counts": np.array([IN_SN_COUNTS[k] for k in ("train", "val", "test")], dtype=np.int64)}
+
+    def store(name, res):
+        for k, vals in zip(keys, zip(*res)):
+            out[name + "/" + k] = np.stack([np.asarray(v.numpy() if torch.is_tensor(v) else v, dtype=np.float32)
+                                            for v in vals])
+        print("indoor_pairs", name, {k: out[name + "/" + k].shape for k in keys})
+
+    with tempfile.TemporaryDirectory() as root:
+        write_synthetic_3dmatch_train(root, IN_M3_LAYOUT, lambda i: IN_M3_ROWS[i], seed=IN_SEED)
+        for name, (mode, rel, seed, S, rh, r3, rp, tp) in IN_M3_CASES.items():
+            opt = ref_shim.make_opt(input_pc_num=IN_N, node_num=IN_M, surface_normal_len=S, rot_horizontal=bool(rh),
+                                    rot_3d=bool(r3), rot_perturbation=bool(rp), translation_perturbation=bool(tp))
+            loader = m3.Match3DDetectorLoader(root, mode, opt)
+            listed = [os.path.relpath(p, root) for p in loader.dataset]
+            np.random.seed(seed)
+            store(name, [loader[listed.index(r)] for r in rel])
+            out[name + "/case"] = np.array([seed, S, rh, r3, rp, tp], dtype=np.int64)
+            out[name + "/paths"] = np.array(rel)
+            out[name + "/mode"] = np.array(mode)
+    with tempfile.TemporaryDirectory() as root:
+        write_synthetic_scenenn(root, IN_SN_COUNTS, indoor_scenenn_rows, seed=IN_SEED)
+        opt = ref_shim.make_opt(input_pc_num=IN_N, node_num=IN_M, surface_normal_len=4, rot_horizontal=False,
+                                rot_3d=True, rot_perturbation=False, translation_perturbation=False)
+        loaders = {split: sn.SceneNNDetectorLoader(root, split, opt) for split in IN_SN_COUNTS}
+        for name, (items, seed) in IN_SN_CASES.items():
+            np.random.seed(seed)
+            store(name, [loaders[split][i] for split, i in items])
+            out[name + "/case"] = np.array([seed, 4, 0, 1, 0, 0], dtype=np.int64)
+            out[name + "/paths"] = np.array(["frames_%s/%d.npy" % (split, i) for split, i in items])
+            out[name + "/mode"] = np.array([split for split, _ in items])
+    np.savez_compressed(os.path.join(OUT, "indoor_pairs.npz"), **out)
+    print("indoor_pairs.npz", os.path.getsize(os.path.join(OUT, "indoor_pairs.npz")) // 1024, "KB")
+
+
 # data/oxford_detector_loader.py OxfordLoader.__getitem__ and data/oxford_descriptor_loader.py OxfordDescriptorLoader
 # (items + default_collate + mine_negative_sample) on a synthetic Oxford tree (usip_b200.data.oxford_detector_loader.
 # write_synthetic_oxford): OX_TRAIN ENU scans along a line (positives within 2, non-negatives within 4), an invalid line

@@ -64,6 +64,9 @@ SIGNATURES = {
     "usip_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                   ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
                           + [c_ptr] * 9 + [c_ptr]),
+    "usip_indoor_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
+                                         ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
+                                 + [c_ptr] * 9 + [c_ptr]),
     "usip_modelnet_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                            ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
                                    + [c_ptr] * 9 + [c_ptr]),

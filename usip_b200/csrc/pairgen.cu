@@ -25,6 +25,7 @@ constexpr int PG_THREADS = 1024;                   // subset kernel: one CTA per
 constexpr int PG_AUG_THREADS = 256;
 constexpr uint32_t PG_SENTINEL = 0xffffffffu;      // key of a point that may not be drawn (outside the radius)
 constexpr int PG_PARAM_STRIDE = 48;                // doubles per pair, see usip_pair_augment in the header
+constexpr int PG_AUGMENT_SLOT = 45;                // usip_indoor_pair_augment: params[b, 45] != 0 augments pair b
 constexpr int PG_DESC_PARAM_STRIDE = 32;           // doubles per cloud, see usip_desc_pair_augment in the header
 constexpr int PG_MAX_PAIRS = 32767;                // 2*n_pairs clouds run in grid.y, at most 65535
 
@@ -423,9 +424,9 @@ __device__ __forceinline__ void pg_augment_point(int flags, const double* P, dou
   }
 }
 
-// sn jitter: fl32(double(sn) + j) with j clipped N(0, 0.01^2), never scaled or shifted; at = the point's row in jit_sn
+// sn jitter: fl32(double(sn) + j) with j clipped N(0, sigma^2), never scaled or shifted; at = the point's row in jit_sn
 __device__ __forceinline__ void pg_jitter_sn(const double* jit_sn, int64_t at, uint64_t seed, uint64_t step, int c,
-                                             int i, int S, float* sn) {
+                                             int i, int S, double sigma, double clip, float* sn) {
 #pragma unroll
   for (int q = 0; q < PG_MAX_S; q += 4) {
     if (q >= S) break;
@@ -437,7 +438,7 @@ __device__ __forceinline__ void pg_jitter_sn(const double* jit_sn, int64_t at, u
       const uint4 u = pg_random(seed, step, c, i, PURPOSE_JIT_SN, q / 4);
       pg_normal2(u.x, u.y, js[0], js[1]); pg_normal2(u.z, u.w, js[2], js[3]);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) js[k] = pg_clip(0.01 * js[k], 0.05);
+      for (int k = 0; k < 4; ++k) js[k] = pg_clip(sigma * js[k], clip);
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k)
@@ -484,19 +485,28 @@ __device__ __forceinline__ void pg_dst_transform(const float* RT, const double* 
   x = __fadd_rn(x, (float)P[40]); y = __fadd_rn(y, (float)P[41]); z = __fadd_rn(z, (float)P[42]);
 }
 
+// The device-mode jitter laws of one augment call: N(0, sigma^2) clipped at +-clip for pc, every sn column and nodes.
+struct PgJitterLaws {
+  double pc_sigma, pc_clip, sn_sigma, sn_clip, node_sigma, node_clip;
+};
+
+// KITTI / Oxford detector pairs (usip_pair_augment) and, with per_pair_switch, the indoor detector pairs
+// (usip_indoor_pair_augment, data/match3d_detector_loader.py / scenenn_detector_loader.py): the same arithmetic, the
+// laws and the sn column passed in.  per_pair_switch: pair b is augmented only when params[b, 45] != 0.
 __global__ void __launch_bounds__(PG_AUG_THREADS)
 pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
                     const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
                     const float* __restrict__ nodes, const double* __restrict__ params,
                     const double* __restrict__ jit_pc, const double* __restrict__ jit_sn,
                     const double* __restrict__ jit_node, uint64_t seed, uint64_t step, int flags, int S, int sn_col,
-                    int N, int M, float* __restrict__ src_pc, float* __restrict__ src_sn, float* __restrict__ src_node,
-                    float* __restrict__ dst_pc, float* __restrict__ dst_sn, float* __restrict__ dst_node,
-                    float* __restrict__ R_out, float* __restrict__ scale_out, float* __restrict__ shift_out) {
+                    PgJitterLaws law, int per_pair_switch, int N, int M, float* __restrict__ src_pc,
+                    float* __restrict__ src_sn, float* __restrict__ src_node, float* __restrict__ dst_pc,
+                    float* __restrict__ dst_sn, float* __restrict__ dst_node, float* __restrict__ R_out,
+                    float* __restrict__ scale_out, float* __restrict__ shift_out) {
   const int c = blockIdx.y, b = c >> 1, side = c & 1;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const double* P = params + (int64_t)b * PG_PARAM_STRIDE;
-  const bool train = flags & USIP_PAIR_TRAIN;
+  const bool train = (flags & USIP_PAIR_TRAIN) && (!per_pair_switch || P[PG_AUGMENT_SLOT] != 0.0);
   float RT[9];
 #pragma unroll
   for (int k = 0; k < 9; ++k) RT[k] = (float)P[31 + k];
@@ -517,9 +527,9 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
     pg_enu_to_cam(flags, P[44], y, z, sn, S);      // Oxford only: height scale, then the camera frame
     if (train) {                                   // KittiLoader.augment, :182-212
       double j[4];
-      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, 0.04, 0.12, j);
+      pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, law.pc_sigma, law.pc_clip, j);
       pg_augment_point(flags, P, P[27], j, S, x, y, z, sn);
-      pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, sn);
+      pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, law.sn_sigma, law.sn_clip, sn);
     }
     float* opc = side ? dst_pc : src_pc;
     float* osn = side ? dst_sn : src_sn;
@@ -541,7 +551,8 @@ pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __res
     pg_enu_to_cam(flags & ~USIP_PAIR_HEIGHT_SCALE, 1.0, y, z, nullptr, 0);
     if (train) {
       double j[4];
-      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, 0.04, 0.12, j);
+      pg_jitter_xyz(jit_node, (int64_t)c * M + i, seed, step, c, i, PURPOSE_JIT_NODE, law.node_sigma, law.node_clip,
+                    j);
       pg_augment_node(flags, P, P[27], j, x, y, z);
     }
     float* ond = side ? dst_node : src_node;
@@ -655,7 +666,7 @@ desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* 
       double j[4];
       pg_jitter_xyz(jit_pc, (int64_t)c * N + i, seed, step, c, i, PURPOSE_JIT_PC, 0.04, 0.12, j);
       pg_augment_point(flags, P, P[27], j, S, x, y, z, sn);
-      pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, sn);
+      pg_jitter_sn(jit_sn, (int64_t)c * N + i, seed, step, c, i, S, 0.01, 0.05, sn);
     }
     float* opc = side ? pos_pc : anc_pc;
     float* osn = side ? pos_sn : anc_sn;
@@ -867,11 +878,35 @@ extern "C" int usip_pair_augment(const float* scans, int C, const int64_t* offse
   USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "pair_augment: bad sizes");
   USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "pair_augment: at most 32767 pairs");
   const int sn_col = S == 1 ? C - 1 : 3;           // kitti_detector_loader.py:135-139
+  const PgJitterLaws kitti = {0.04, 0.12, 0.01, 0.05, 0.04, 0.12};   // kitti_detector_loader.py:164-172
   dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
   pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
-      scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, sn_col, N,
-      M, src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, R, scale, shift);
+      scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, sn_col,
+      kitti, 0, N, M, src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, R, scale, shift);
   return check_launch("pair_augment_kernel");
+}
+
+extern "C" int usip_indoor_pair_augment(const float* scans, int C, const int64_t* offsets,
+                                        const int32_t* scan_of_cloud, const int32_t* rows, const float* nodes,
+                                        const double* params, const double* jit_pc, const double* jit_sn,
+                                        const double* jit_node, uint64_t seed, uint64_t step, int flags, int S,
+                                        int n_pairs, int N, int M, float* src_pc, float* src_sn, float* src_node,
+                                        float* dst_pc, float* dst_sn, float* dst_node, float* R, float* scale,
+                                        float* shift, void* stream) {
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && nodes && params, "indoor_pair_augment: null input");
+  USIP_REQUIRE(src_pc && src_sn && src_node && dst_pc && dst_sn && dst_node && R && scale && shift,
+               "indoor_pair_augment: null output");
+  USIP_REQUIRE(S >= 1 && S <= PG_MAX_S && 3 + S <= C, "indoor_pair_augment: sn is columns 3:3+S (1 <= S <= 8, 3+S <= C)");
+  USIP_REQUIRE(!(flags & (USIP_PAIR_ENU_TO_CAM | USIP_PAIR_HEIGHT_SCALE)),
+               "indoor_pair_augment: the Oxford frame flags do not apply to indoor fragments");
+  USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0, "indoor_pair_augment: bad sizes");
+  USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "indoor_pair_augment: at most 32767 pairs");
+  const PgJitterLaws indoor = {0.01, 0.02, 0.01, 0.02, 0.01, 0.02};  // match3d_detector_loader.py:125-132
+  dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
+  pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
+      scans, C, offsets, scan_of_cloud, rows, nodes, params, jit_pc, jit_sn, jit_node, seed, step, flags, S, 3, indoor,
+      1, N, M, src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, R, scale, shift);
+  return check_launch("pair_augment_kernel(indoor)");
 }
 
 extern "C" int usip_modelnet_pair_augment(const float* scans, int C, const int64_t* offsets,

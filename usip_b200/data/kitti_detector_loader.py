@@ -4,8 +4,9 @@
 whole training batch of `KittiLoader.__getitem__` (:218-259) on the device -- random subsampling, FPS nodes,
 augmentation and the dst transform -- and `KittiPairSource` feeds such batches to `ModelDetector` from a KITTI tree.
 The reference runs all of this per pair in DataLoader workers: serial numpy, more host time per pair than a whole
-training step of this repository.  The KITTI loaders, the ModelNet detector loader (modelnet_shrec_loader.py) and the
-Oxford loaders (oxford_detector_loader.py, oxford_descriptor_loader.py) build on the bases here.
+training step of this repository.  The KITTI loaders, the ModelNet detector loader (modelnet_shrec_loader.py), the
+Oxford loaders (oxford_detector_loader.py, oxford_descriptor_loader.py) and the 3DMatch and SceneNN detector loaders
+(match3d_detector_loader.py, scenenn_detector_loader.py) build on the bases here.
 """
 import os
 
@@ -61,36 +62,53 @@ def radius_mask(pc, radius):
     return np.linalg.norm(pc[:, [0, 2]], axis=1) <= radius
 
 
+def draw_rows(rng, n_valid, N):
+    """The row draws of get_instance_unaugmented_np (:126-137) for one cloud: N rows of the n_valid (masked) points,
+    without replacement, or every point t times and a random remainder when there are fewer than N."""
+    if n_valid >= N:
+        return rng.choice(n_valid, N, replace=False)
+    fix = np.arange(n_valid)
+    while n_valid + fix.shape[0] < N:
+        fix = np.concatenate((fix, np.arange(n_valid)), axis=0)
+    return np.concatenate((fix, rng.choice(n_valid, N - fix.shape[0], replace=False)), axis=0)
+
+
+def draw_candidates(rng, N, divisor):
+    """The FPS draws of one cloud: candidate positions into its N rows, then FarthestSampler.sample's start (:78)."""
+    cand = rng.choice(N, int(N / divisor), replace=False)
+    return cand, rng.randint(len(cand))
+
+
 def draw_subsample(rng, n_valid, N, divisor=3):
     """The index draws of get_instance_unaugmented_np (:126-145) for one cloud, in the reference's order:
     rows into the n_valid (masked) points, FPS candidate positions into the N rows, FPS start."""
-    if n_valid >= N:
-        choice = rng.choice(n_valid, N, replace=False)
-    else:
-        fix = np.arange(n_valid)
-        while n_valid + fix.shape[0] < N:
-            fix = np.concatenate((fix, np.arange(n_valid)), axis=0)
-        choice = np.concatenate((fix, rng.choice(n_valid, N - fix.shape[0], replace=False)), axis=0)
-    cand = rng.choice(N, int(N / divisor), replace=False)
-    start = rng.randint(len(cand))                                  # FarthestSampler.sample, :78
-    return choice, cand, start
+    choice = draw_rows(rng, n_valid, N)
+    return (choice,) + draw_candidates(rng, N, divisor)
 
 
-def draw_pair_scalars(rng, opt, train, N, M, S, per_point, scale_range=(0.9, 1.1)):
+KITTI_PERTURBATION = (0.06, 0.18)                # kitti_detector_loader.py:160: sigma and clip of the angles
+KITTI_JITTER = ((0.04, 0.12), (0.01, 0.05), (0.04, 0.12))   # :164-172: pc, sn, node
+
+
+def draw_pair_scalars(rng, opt, train, N, M, S, per_point, scale_range=(0.9, 1.1), perturbation=KITTI_PERTURBATION,
+                      jitter=KITTI_JITTER, scale_thre=0.0):
     """Scalars of augment() (:157-175, train only) and transform_pc_pytorch (augmentation.py:210-243) for one pair,
     in the reference's order -> (params (48,) f64, jitter (pc (2,N,3), sn (2,N,S), node (2,M,3)) or None).
-    per_point=False skips the O(N) jitter draws (the device draws its own).  scale_range: the augmentation scale's
-    uniform law, KITTI's by default (the Oxford detector's is (0.7, 1.3))."""
+    per_point=False skips the O(N) jitter draws (the device draws its own).  The laws default to KITTI's: scale_range
+    the augmentation scale's uniform law (the Oxford detector's is (0.7, 1.3)), perturbation the (sigma, clip) of the
+    augmentation's perturbation angles, jitter the (sigma, clip) of pc, sn and node, scale_thre the transform's scale
+    range 1 +- scale_thre (the indoor loaders' laws are in match3d_detector_loader.py)."""
     p = np.zeros(ops.PAIR_PARAM_STRIDE, dtype=np.float64)
     jit = None
     if train:
         y_angle = rng.uniform() * 2 * np.pi
         angles_2d = [0, y_angle, 0]
         angles_3d = rng.rand(3) * np.pi * 2
-        angles_pertb = np.clip(0.06 * rng.randn(3), -0.18, 0.18)
+        angles_pertb = np.clip(perturbation[0] * rng.randn(3), -perturbation[1], perturbation[1])
         if per_point:
-            jit = (np.clip(0.04 * rng.randn(2, N, 3), -0.12, 0.12), np.clip(0.01 * rng.randn(2, N, S), -0.05, 0.05),
-                   np.clip(0.04 * rng.randn(2, M, 3), -0.12, 0.12))
+            (ps, pc), (ss, sc), (ns, nc) = jitter
+            jit = (np.clip(ps * rng.randn(2, N, 3), -pc, pc), np.clip(ss * rng.randn(2, N, S), -sc, sc),
+                   np.clip(ns * rng.randn(2, M, 3), -nc, nc))
         scale = rng.uniform(low=scale_range[0], high=scale_range[1])
         shift = rng.uniform(-1, 1, (1, 3))
         p[0:9] = angles2rotation_matrix(angles_2d).ravel()
@@ -115,7 +133,7 @@ def draw_pair_scalars(rng, opt, train, N, M, S, per_point, scale_range=(0.9, 1.1
         y_angle += np.clip(angle_sigma * rng.randn(), -angle_clip, angle_clip)
         z_angle += np.clip(angle_sigma * rng.randn(), -angle_clip, angle_clip)
     p[31:40] = angles2rotation_matrix([x_angle, y_angle, z_angle]).astype(np.float32).ravel()
-    scale_t = rng.uniform(low=1 - 0, high=1 + 0)                   # scale_thre = 0
+    scale_t = rng.uniform(low=1 - scale_thre, high=1 + scale_thre)  # KITTI: scale_thre = 0
     p[40:43] = rng.uniform(-0.5, 0.5, (3, 1)).astype(np.float32).ravel()
     p[43] = np.float32(scale_t)
     return p, jit
@@ -214,9 +232,12 @@ class _PairBuilder:
         if scans.dim() != 2 or C < 3 + max(S, 1):
             raise ValueError("scans have %d columns, surface_normal_len %d needs %d" % (C, S, 3 + S))
         max_rows = int(max(lengths.max(), N))
-        if max_rows > ops.pair_max_scan_rows():
-            raise ValueError("a scan of %d rows exceeds the %d the subsample kernel holds"
-                             % (max_rows, ops.pair_max_scan_rows()))
+        if N > ops.pair_max_scan_rows():
+            raise ValueError("input_pc_num %d exceeds the %d rows the subsample kernel holds"
+                             % (N, ops.pair_max_scan_rows()))
+        if max_rows > ops.SUBSAMPLE_MAX_ROWS:
+            raise ValueError("a scan of %d rows exceeds the %d the subsample kernels take"
+                             % (max_rows, ops.SUBSAMPLE_MAX_ROWS))
         if step is None:
             step = self.step
         self.step = int(step) + 1
@@ -369,12 +390,15 @@ def synthetic_scan(seed, Ns, C=8):
 
 class _ScanSource:
     """What every device-built pair source shares, whatever its tree: a list of `.npy` scans (`paths[i]` is the scan of
-    item i, unless a subclass indexes them itself) loaded once into pinned host memory, or onto the device with resident="device"; shuffled epochs; and the
+    item i, unless a subclass indexes them itself) loaded once into pinned host memory, or onto the device with
+    resident="device", or (subclasses with `disk_resident`) read from disk batch by batch with resident="disk"; shuffled epochs; and the
     hand-over.  Iteration builds batch i+1 on a stream of its own while the caller runs step i, and hands each batch over
     with `model.prefetch_input(..., after=event)` + `set_input()`: the model's stream waits on the build's event, the
     host never synchronises.  Every batch is a fresh set of tensors, so a batch still in use is never overwritten.  A
     subclass turns the item indices of one batch into the model's inputs (`_build`, called with the build stream
     current)."""
+
+    disk_resident = False                        # whether the subclass's _build reads scans through _batch_scans
 
     def __init__(self, paths, mode, opt, builder, device, seed, resident, rng, batch_size, drop_last, n_items=None):
         self.opt, self.mode = opt, mode
@@ -382,12 +406,18 @@ class _ScanSource:
         self.device = torch.device(device if device is not None else "cuda")
         self.batch_size = int(batch_size or opt.batch_size)
         self.drop_last = drop_last
-        arrs = [load_scan_npy(p, opt.surface_normal_len) for p in paths]
-        if len({a.shape[1] for a in arrs}) != 1:
-            raise ValueError("scans differ in column count")
-        self.offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrs])]).astype(np.int64)
-        scans = torch.from_numpy(np.concatenate(arrs))
-        self.scans = scans.to(self.device) if resident == "device" else scans.pin_memory()
+        if resident == "disk" and not self.disk_resident:
+            raise ValueError("resident='disk' is not supported by %s" % type(self).__name__)
+        self.paths = list(paths)
+        if resident == "disk":                   # only the file list; each batch loads its own scans
+            self.scans = self.offsets = None
+        else:
+            arrs = [load_scan_npy(p, opt.surface_normal_len) for p in paths]
+            if len({a.shape[1] for a in arrs}) != 1:
+                raise ValueError("scans differ in column count")
+            self.offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrs])]).astype(np.int64)
+            scans = torch.from_numpy(np.concatenate(arrs))
+            self.scans = scans.to(self.device) if resident == "device" else scans.pin_memory()
         self.builder = builder(opt, mode, self.device, seed, rng)
         self.order_rng = np.random.RandomState(seed)
         self.stream = torch.cuda.Stream(device=self.device)
@@ -401,6 +431,20 @@ class _ScanSource:
     def _build(self, items):
         """-> (the model's input tensors, what `last` will say about them)."""
         raise NotImplementedError
+
+    def _batch_scans(self, scan_idx):
+        """(scans, offsets, scan index into them) for a batch naming scans scan_idx.  Resident scans are returned as
+        they are; with resident="disk" the batch's scans are loaded now, each once, in ascending index order -- the
+        order in which the builder uploads host scans, so both give the same batch bit for bit."""
+        scan_idx = np.asarray(scan_idx, dtype=np.int64)
+        if self.scans is not None:
+            return self.scans, self.offsets, scan_idx
+        used, inv = np.unique(scan_idx, return_inverse=True)
+        arrs = [load_scan_npy(self.paths[i], self.opt.surface_normal_len) for i in used]
+        if len({a.shape[1] for a in arrs}) != 1:
+            raise ValueError("scans differ in column count")
+        offsets = np.concatenate([[0], np.cumsum([len(a) for a in arrs])]).astype(np.int64)
+        return torch.from_numpy(np.concatenate(arrs)).pin_memory(), offsets, inv.reshape(scan_idx.shape)
 
     def _enqueue(self, items):
         with torch.cuda.stream(self.stream):

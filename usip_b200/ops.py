@@ -142,6 +142,7 @@ def fps(pts, start, k, want_nodes=True):
 PAIR_TRAIN, PAIR_ROT_HORIZONTAL, PAIR_ROT_3D, PAIR_ROT_PERTURBATION, PAIR_TRANSLATION = 1, 2, 4, 8, 16
 PAIR_ENU_TO_CAM, PAIR_HEIGHT_SCALE = 32, 64      # Oxford: camera frame first; detector height scale = params[:, 44]
 PAIR_PARAM_STRIDE = 48                           # detector: doubles per pair
+PAIR_AUGMENT_SLOT = 45                           # indoor_pair_augment: params[:, 45] != 0 augments the pair
 SUBSAMPLE_MAX_ROWS = 1 << 24                     # cloud_subsample: the longest scan (USIP_SUBSAMPLE_MAX_ROWS)
 DESC_PARAM_STRIDE = 32                           # descriptor: doubles per cloud
 
@@ -235,6 +236,25 @@ def pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, S, flags, s
             _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows), _p(nodes), _p(params), _p(jit_pc),
             _p(jit_sn), _p(jit_node), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), int(flags), int(S), B, N, M,
             *[_p(t) for t in out], _stream()), "usip_pair_augment")
+    return out
+
+
+def indoor_pair_augment(scans, offsets, scan_of_cloud, rows, nodes, params, S, flags, seed=0, step=0, jit_pc=None,
+                        jit_sn=None, jit_node=None):
+    """3DMatch / SceneNN detector augmentation + dst transform -> the nine ModelDetector.set_input tensors, as
+    pair_augment but with the indoor jitter laws (sigma 0.01, clip 0.02 for pc, sn and nodes), sn = scan columns 3:3+S
+    for every S, and a per-pair switch: with PAIR_TRAIN, pair b is augmented only when params[b, PAIR_AUGMENT_SLOT] != 0.
+    Jitter arrays per cloud, (2B, N, 3), (2B, N, S), (2B, M, 3) f64, or None (drawn on the device from (seed, step))."""
+    _req_scans(scans, offsets, scan_of_cloud); _req(rows, i32, "rows"); _req(nodes, f32, "nodes")
+    _req(params, torch.float64, "params"); _req_jitter(jit_pc, jit_sn, jit_node)
+    B, N, M, dev = scan_of_cloud.shape[0] // 2, rows.shape[1], nodes.shape[2], scans.device
+    e = lambda *s: torch.empty(s, dtype=f32, device=dev)
+    out = (e(B, 3, N), e(B, S, N), e(B, 3, M), e(B, 3, N), e(B, S, N), e(B, 3, M), e(B, 3, 3), e(B), e(B, 3, 1))
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_indoor_pair_augment(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows), _p(nodes), _p(params), _p(jit_pc),
+            _p(jit_sn), _p(jit_node), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), int(flags), int(S), B, N, M,
+            *[_p(t) for t in out], _stream()), "usip_indoor_pair_augment")
     return out
 
 
