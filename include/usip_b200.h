@@ -446,6 +446,14 @@ int usip_knn_combine(const float* Z, int ldz, const float* pts, const int32_t* k
 int usip_group_select(const float* gmax, const float* gmin, const float* scale, const float* shift,
                       float* out, int ldo, int Q, int C, void* stream);
 
+/* Groups larger than the layer epilogue's 128 rows: out_max[q, c] = max over r < ratio of gmax[q*ratio + r, c] (and
+ * out_min likewise from gmin, when both are given) for Q_out x C outputs, rows contiguous ([Q_out*ratio, C] in,
+ * [Q_out, C] out).  Same comparison as the epilogue's group max (strict >, strict <, from -inf / +inf; NaN never wins)
+ * and the result of one in-order scan, so it is deterministic.  The indoor descriptor uses it for its 448-row balls
+ * (64-row sub-groups, ratio 7) and for the per-cloud global max over its M keypoints (ratio M).  No arg outputs. */
+int usip_group_max_combine(const float* gmax, const float* gmin, float* out_max, float* out_min, int ratio, int Q_out,
+                           int C, void* stream);
+
 /* networks.py:151-154: keypoints (B,3,M) = out[:, :3] + cluster_mean ; sigmas (B,M) = softplus(out[:,3]) + lb */
 int usip_head_finalize(const float* out4, int ld, const float* cluster_mean, float sigma_lower_bound,
                        float* keypoints, float* sigmas, int B, int M, void* stream);

@@ -178,6 +178,39 @@ def golden_descriptor(ref):
     np.savez_compressed(os.path.join(OUT, "descriptor.npz"), **out)
 
 
+def golden_descriptor_indoor(ref):
+    """DescriptorLiteOldGlobal (models/networks.py:388-479) on the CPU, with tests/desc_indoor_ref.py supplying the
+    operations.ball_query_wrapper the reference ships commented out: eval and train BatchNorm, the running statistics
+    after the train forward, the ball indices and a fixed sample of x_features."""
+    from tests import desc_indoor_ref as dref
+    B, N, M, S, K, seed, D, radius = 2, 2048, 64, 4, 448, 81, 64, 0.75
+    pc, sn, kp = dref.make_inputs(B, N, M, S, seed, half=1.0)
+    opt = ref_shim.make_opt(batch_size=B, input_pc_num=N, node_num=M, surface_normal_len=S, ball_radius=radius,
+                            ball_nsamples=K, descriptor_len=D)
+    torch.manual_seed(seed)
+    params = dref.randomized_params(ref.networks.DescriptorLiteOldGlobal(opt), seed)
+    case = dict(cfg=np.array([B, N, M, S, K, seed], np.int64), radius=np.float32(radius), D=np.int64(D), pc=pc, sn=sn,
+                kp=kp, **{"param/" + k: v.numpy() for k, v in params.items()})
+    out = dref.reference_outputs(ref, _NpzLike(case))
+    assert np.array_equal(out["eval_feats"], out["train_feats"])
+    perm = np.random.RandomState(seed).permutation(N)
+    dist = np.linalg.norm(kp[:, :, :, None] - pc[:, :, perm][:, :, None, :], axis=1)
+    idx = orc.ball_query_dist(np.ascontiguousarray(dist, dtype=np.float32), radius, K)
+    assert np.array_equal(dref.reconstruct_features(pc, sn, kp, idx, perm), out["eval_feats"])
+    hits = (dist <= np.float32(radius)).sum(2)
+    print("descriptor_indoor: ball hits min %d median %d max %d (K=%d)" % (hits.min(), np.median(hits), hits.max(), K))
+    case.update(perm=perm.astype(np.int64), idx=idx.astype(np.int16),
+                feats=out["eval_feats"].ravel()[dref.feats_sample(out["eval_feats"].size)], eval_desc=out["eval_desc"], train_desc=out["train_desc"],
+                **{k: v for k, v in out.items() if k.startswith("after/")})
+    np.savez_compressed(os.path.join(OUT, "descriptor_indoor.npz"), **case)
+
+
+class _NpzLike(dict):
+    @property
+    def files(self):
+        return list(self.keys())
+
+
 def golden_descriptor_train(ref):
     """One ModelDescriptor.optimize() of the reference (keypoint_descriptor.py:126-157) on CPU: loss, gradient
     summaries, post-Adam parameter summaries.  Inputs are regenerated from the seed by the consumers."""
@@ -810,6 +843,7 @@ def main():
     golden_descriptor(ref)
     golden_desc_loss(ref)
     golden_descriptor_train(ref)
+    golden_descriptor_indoor(ref)
     golden_fps(ref)
     golden_nms(ref)
     golden_ablation(ref)

@@ -115,18 +115,47 @@ def descriptor_golden(ref, out):
     np.savez_compressed(os.path.join(out, "reference_descriptor.npz"), **T.descriptor_run(net, x, s, k))
 
 
+def descriptor_indoor_golden(ref, out):
+    """DescriptorLiteOldGlobal at the indoor evaluation shape, with tests/desc_indoor_ref.py's ball_query_wrapper on the
+    reference's ball_query extension: fixed samples of descriptors and x_features, the running statistics whole."""
+    from tests import desc_indoor_ref as dref
+    from tests import test_gpu_descriptor_indoor as DI
+    c = DI.FULL
+    _, (pc, sn, kp), state = DI.full_setup()
+    case = dict(cfg=np.array([c["B"], c["N"], c["M"], c["S"], c["K"], c["seed"]], np.int64), radius=np.float32(0.75),
+                D=np.int64(c["D"]), pc=pc, sn=sn, kp=kp, **{"param/" + k: v.numpy() for k, v in state.items()})
+
+    class Case(dict):
+        files = property(lambda self: list(self.keys()))
+    r = dref.reference_outputs(ref, Case(case))
+    g = {}
+    for mode in ("eval", "train"):
+        g["desc_" + mode], g["feats_" + mode] = DI.sampled(r[mode + "_desc"], r[mode + "_feats"])
+    for k, v in r.items():
+        if k.startswith("after/") and "running" in k:
+            g["run__" + k[len("after/"):]] = v
+    np.savez_compressed(os.path.join(out, "reference_descriptor_indoor.npz"), **g)
+
+
 def main():
     out = sys.argv[1]
+    only = sys.argv[2:]                        # e.g. `descriptor_indoor`: regenerate that file only
     os.makedirs(out, exist_ok=True)
     if not (ref_shim.reference_available() and build_ref.have("index_max") and build_ref.have("ball_query")):
         raise SystemExit("oracle/_ref (the original code's extensions and Python tree) is not built")
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
+    if only:
+        ref = ref_shim.modules(mode="cuda")
+        for name in only:
+            globals()[name + "_golden"](ref, out)
+        return
     ops_golden(out)
     ref = ref_shim.modules(mode="cuda")
     for name in T.CONFIGS:
         detector_golden(ref, name, out)
     descriptor_golden(ref, out)
+    descriptor_indoor_golden(ref, out)
     for f in sorted(os.listdir(out)):
         print(f, os.path.getsize(os.path.join(out, f)))
 

@@ -109,6 +109,7 @@ SIGNATURES = {
     "usip_knn_combine": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_int, c_ptr, c_ptr, c_int, c_ptr,
                                  c_int, c_int, c_int, c_int, c_ptr]),
     "usip_group_select": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
+    "usip_group_max_combine": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_head_finalize": (c_int, [c_ptr, c_int, c_ptr, c_f32, c_ptr, c_ptr, c_int, c_int, c_ptr]),
     "usip_l2norm_to_bcm": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_pairwise_min_f32": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),

@@ -436,6 +436,56 @@ __global__ void group_select4_kernel(const float* __restrict__ gmax, const float
   *reinterpret_cast<float4*>(out + (size_t)q * ldo + c) = o;
 }
 
+// Row q of the output is the max (min) over input rows q*ratio .. q*ratio+ratio-1.  One CTA per (output row, 128-column
+// slab): warp w scans a contiguous slice of those rows, lane l holds columns l, l+32, l+64, l+96 of the slab (coalesced
+// for any C), then warp 0 merges the slices in row order.  Every comparison is the layer epilogue's strict `v > best` /
+// `v < best` from -inf / +inf, and a later slice only replaces an earlier one when strictly better, so the result is
+// that of one in-order scan: deterministic, independent of the launch shape.
+constexpr int GMC_WARPS = 8;
+__global__ void __launch_bounds__(GMC_WARPS * 32)
+group_max_combine_kernel(const float* __restrict__ gmax, const float* __restrict__ gmin, float* __restrict__ omax,
+                         float* __restrict__ omin, int ratio, int C) {
+  __shared__ float smax[GMC_WARPS][128], smin[GMC_WARPS][128];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const size_t q = blockIdx.x;
+  const int c0 = blockIdx.y * 128 + lane;
+  const int per = (ratio + GMC_WARPS - 1) / GMC_WARPS;
+  const int r0 = min(ratio, w * per), r1 = min(ratio, r0 + per);
+  float mx[4], mn[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) { mx[j] = -INFINITY; mn[j] = INFINITY; }
+#pragma unroll 4
+  for (int r = r0; r < r1; ++r) {                              // unrolled: several rows' loads in flight (ratio M)
+    const size_t row = (q * ratio + r) * (size_t)C;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int c = c0 + 32 * j;
+      if (c < C) {
+        const float a = __ldg(gmax + row + c);
+        if (a > mx[j]) mx[j] = a;
+        if (gmin) { const float b = __ldg(gmin + row + c); if (b < mn[j]) mn[j] = b; }
+      }
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) { smax[w][lane + 32 * j] = mx[j]; smin[w][lane + 32 * j] = mn[j]; }
+  __syncthreads();
+  if (w != 0) return;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int c = c0 + 32 * j;
+    if (c >= C) continue;
+    float a = smax[0][lane + 32 * j], b = smin[0][lane + 32 * j];
+    for (int s = 1; s < GMC_WARPS; ++s) {
+      const float x = smax[s][lane + 32 * j], y = smin[s][lane + 32 * j];
+      if (x > a) a = x;
+      if (y < b) b = y;
+    }
+    omax[q * C + c] = a;
+    if (omin) omin[q * C + c] = b;
+  }
+}
+
 __global__ void head_finalize_kernel(const float* __restrict__ out4, int ld, const float* __restrict__ cmean,
                                      float lb, float* __restrict__ kp, float* __restrict__ sig, int B, int M) {
   int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -679,6 +729,16 @@ extern "C" int usip_group_select(const float* gmax, const float* gmin, const flo
   }
   group_select_kernel<<<(unsigned)cdiv64(n, 256), 256, 0, (cudaStream_t)stream>>>(gmax, gmin, scale, shift, out, ldo, Q, C);
   return check_launch("group_select_kernel");
+}
+
+extern "C" int usip_group_max_combine(const float* gmax, const float* gmin, float* out_max, float* out_min, int ratio,
+                                      int Q_out, int C, void* stream) {
+  USIP_REQUIRE(gmax && out_max && !gmin == !out_min, "group_max_combine: bad args (gmin and out_min come together)");
+  USIP_REQUIRE(ratio >= 1 && Q_out >= 1 && C >= 1, "group_max_combine: ratio, Q_out and C must be positive");
+  USIP_REQUIRE(cdiv(C, 128) <= 65535, "group_max_combine: C too large");
+  dim3 grid((unsigned)Q_out, (unsigned)cdiv(C, 128));
+  group_max_combine_kernel<<<grid, GMC_WARPS * 32, 0, (cudaStream_t)stream>>>(gmax, gmin, out_max, out_min, ratio, C);
+  return check_launch("group_max_combine_kernel");
 }
 
 extern "C" int usip_head_finalize(const float* out4, int ld, const float* cluster_mean, float sigma_lower_bound,

@@ -636,15 +636,23 @@ def _group_net_forward(R, net, rows, Bp, M, K, keep, out=None):
         conv1 -> conv2 -> conv3 -> max_k -> conv4 on cat(y, broadcast max) -> conv5 -> max_k
     on point-major rows [Bp*M*K, ld] of the gathered, decentred groups.  conv1..conv4 carry BN+ReLU; conv5 is linear in the
     descriptor (the raw group max is returned) and BN+ReLU in the detectors (max_k relu(bn(.)) is written to `out`).
-    The reference calls these convolutions WITHOUT epoch: their BN momentum never decays."""
+    The reference calls these convolutions WITHOUT epoch: their BN momentum never decays.
+    Balls of more than 128 rows (K a multiple of 64) take the layer epilogue's group max over 64-row sub-groups and reduce
+    each run of K/64 of them with usip_group_max_combine; that path has no arg outputs, so it is forward-only."""
     dev = rows.device
     G, Q = Bp * M * K, Bp * M
+    sub = K if K <= 128 else 64
+    if sub != K and (K % sub != 0 or keep):
+        raise NotImplementedError("group of %d rows: groups above 128 must be a multiple of 64 and run forward only" % K)
     c1, c2, c3, c4, c5 = net.conv1, net.conv2, net.conv3, net.conv4, net.conv5
     D = c3.conv.weight.shape[0]
     Y1, bn1, _ = R.run(rows, G, _w2d(c1.conv.weight), c1.conv.bias.detach(), c1.norm, c1.norm.momentum, name="grp.conv1")
     Y2, bn2, _ = R.run(Y1, G, _w2d(c2.conv.weight), c2.conv.bias.detach(), c2.norm, c2.norm.momentum, prev=bn1, name="grp.conv2")
     Y3, bn3, grp3 = R.run(Y2, G, _w2d(c3.conv.weight), c3.conv.bias.detach(), c3.norm, c3.norm.momentum, prev=bn2,
-                          group=K, want_group=True, want_arg=keep, name="grp.conv3")
+                          group=sub, want_group=True, want_arg=keep, name="grp.conv3")
+    if sub != K:
+        with _Prof("group_max_combine"):
+            grp3["gmax"], grp3["gmin"] = ops.group_max_combine(grp3["gmax"], K // sub, grp3["gmin"])
     amax = torch.empty((Q, D), dtype=f32, device=dev)
     ops.group_select(grp3["gmax"], grp3["gmin"], bn3.scale, bn3.shift, amax, Q, D)          # y_first_max (networks.py:377)
     W4 = _w2d(c4.conv.weight)
@@ -654,8 +662,11 @@ def _group_net_forward(R, net, rows, Bp, M, K, keep, out=None):
                        add_group=K, name="grp.conv4")
     last_bn = getattr(c5, "norm", None) is not None
     Y5, bn5, grp5 = R.run(Y4, G, _w2d(c5.conv.weight), c5.conv.bias.detach(), c5.norm if last_bn else None,
-                          c5.norm.momentum if last_bn else 0.1, prev=bn4, group=K, want_group=True, want_arg=keep,
+                          c5.norm.momentum if last_bn else 0.1, prev=bn4, group=sub, want_group=True, want_arg=keep,
                           write_y=last_bn and keep, name="grp.conv5")
+    if sub != K:
+        with _Prof("group_max_combine"):
+            grp5["gmax"], grp5["gmin"] = ops.group_max_combine(grp5["gmax"], K // sub, grp5["gmin"] if last_bn else None)
     result = grp5["gmax"]
     if last_bn:
         C5 = c5.conv.weight.shape[0]
@@ -732,18 +743,9 @@ def descriptor_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=True, k
     if keep and not net.training:
         raise NotImplementedError("gradients through eval-mode BatchNorm are not part of the hot path "
                                   "(the reference only back-propagates in train mode, keypoint_descriptor.py:138)")
-    Bp, _, N = x.shape
-    M = keypoints.shape[2]
-    K = opt.ball_nsamples
-    S = opt.surface_normal_len if opt.surface_normal_len > 0 else 0
-    G, Q = Bp * M * K, Bp * M
+    Bp, M, K = x.shape[0], keypoints.shape[2], opt.ball_nsamples
     R = LayerRunner(net, net.training, use_tc, dev)
-    # permute the points on the host-drawn permutation: the ball query keeps the FIRST K hits in index order
-    x = x.detach()[:, :, permute_idx].contiguous()
-    snp = sn.detach()[:, :, permute_idx].contiguous() if S else None
-    kp = keypoints.detach().contiguous()
-    with _Prof("ball_group", nbytes=4.0 * Bp * (N * (3 + S) + 3 * M + M * K + (3 + S) * M * K)):
-        idx, feats, rows = ops.ball_group(x, snp, kp, float(opt.ball_radius), K, want_group=True, rows_ld=8)
+    feats, rows = _descriptor_balls(opt, x, sn, keypoints, permute_idx)
     gmax5, gctx = _group_net_forward(R, net, rows, Bp, M, K, keep, out=None)
     D = gctx["D"]
     desc = torch.empty((Bp, D, M), dtype=f32, device=dev)
@@ -754,6 +756,52 @@ def descriptor_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=True, k
         ctx = dict(gctx)
         ctx.update(use_tc=use_tc)
     return desc, feats, ctx
+
+
+def _descriptor_balls(opt, x, sn, keypoints, permute_idx):
+    """networks.py:345-373: the balls of both descriptors -> (x_features (B,3+S,M,K), point-major rows [B*M*K, 8])."""
+    Bp, _, N = x.shape
+    M = keypoints.shape[2]
+    K = opt.ball_nsamples
+    S = opt.surface_normal_len if opt.surface_normal_len > 0 else 0
+    # permute the points on the host-drawn permutation: the ball query keeps the FIRST K hits in index order
+    x = x.detach()[:, :, permute_idx].contiguous()
+    snp = sn.detach()[:, :, permute_idx].contiguous() if S else None
+    kp = keypoints.detach().contiguous()
+    with _Prof("ball_group", nbytes=4.0 * Bp * (N * (3 + S) + 3 * M + M * K + (3 + S) * M * K)):
+        _, feats, rows = ops.ball_group(x, snp, kp, float(opt.ball_radius), K, want_group=True, rows_ld=8)
+    return feats, rows
+
+
+def descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=True):
+    """DescriptorLiteOldGlobal.forward (models/networks.py:433-479) on the fused plan, forward only.  The grouped PointNet
+    is DescriptorLiteOld's; then PPFNet's global context:
+        g = max over the M keypoints of each cloud of the raw conv5 max          (usip_group_max_combine, ratio M)
+        fc1 on cat(desc, g) = desc W1[:, :D]^T + (g W1[:, D:]^T)[row / M] + b  -> BN + ReLU
+        fc2 -> BN + ReLU, fc3 linear, L2 normalisation.
+    The EquivariantLayers are called without epoch, like the convolutions: their BN momentum never decays.
+    Returns (descriptor (B,D,M), x_features (B,3+S,M,K))."""
+    opt = net.opt
+    dev = x.device
+    Bp, M, K = x.shape[0], keypoints.shape[2], opt.ball_nsamples
+    Q = Bp * M
+    R = LayerRunner(net, net.training, use_tc, dev)
+    feats, rows = _descriptor_balls(opt, x, sn, keypoints, permute_idx)
+    local, gctx = _group_net_forward(R, net, rows, Bp, M, K, False, out=None)        # [Q, D] raw max of conv5
+    D = gctx["D"]
+    with _Prof("global_max"):
+        glob, _ = ops.group_max_combine(local, M)                                     # [Bp, D]
+    f1, f2, f3 = net.fc1, net.fc2, net.fc3
+    W1 = _w2d(f1.conv.weight)
+    U, _, _ = R.run(glob, Bp, _cols(W1, D), None, relu_in=False, name="fc1_global")   # cat(desc, global): global is LAST
+    Y1, bn1, _ = R.run(local, Q, _cols(W1, 0, D), f1.conv.bias.detach(), f1.norm, f1.norm.momentum, relu_in=False,
+                       addend=U, add_group=M, name="fc1")
+    Y2, bn2, _ = R.run(Y1, Q, _w2d(f2.conv.weight), f2.conv.bias.detach(), f2.norm, f2.norm.momentum, prev=bn1, name="fc2")
+    OUT, _, _ = R.run(Y2, Q, _w2d(f3.conv.weight), f3.conv.bias.detach(), prev=bn2, name="fc3")
+    desc = torch.empty((Bp, OUT.shape[1], M), dtype=f32, device=dev)
+    _lib.check(_lib.load().usip_l2norm_to_bcm(ops._p(OUT), OUT.stride(0), ops._p(desc), None, Bp, M, OUT.shape[1],
+                                              ops._stream()), "usip_l2norm_to_bcm")
+    return desc, feats
 
 
 def _group_net_backward(bw, net, ctx, GY5):

@@ -4,7 +4,7 @@ writeLog.m, evaluate.m -> mrEvaluateRegistrationMy.m), for the Redwood and 3DMat
 sweep and every maxTrials of a sweep at once.
 
     ev = IndoorRegistration.redwood(npy_root, gt_root, descriptor_opt("redwood"))
-    ev.read_descriptor_tree(tree, 128)            # or ev.describe(detector, descriptor)
+    ev.read_descriptor_tree(tree, 128)            # or ev.describe(detector, ModelDescriptorIndoor)
     res = ev.score()
     print("\\n".join(res.lines()))
     ev.write_registration_logs(out_dir, K=512, max_trials=30000)
@@ -30,6 +30,12 @@ Deliberate deviations from the reference:
   * The .log is written straight from the kernels' fp64 results (%.10f), not re-read from the %15.8e of a per-pair
     .rt.txt.
   * 3DMatch fragments are taken in frame order (indoor_test_loader.py).
+
+Descriptors (describe, with a ModelDescriptorIndoor): DescriptorLiteOldGlobal's global context is the max over the
+keypoints the descriptor is given.  describe() gives it all M keypoints of the detector pass, before NMS and before the
+top-K selection -- the keypoint set scenenn/train_descriptor.py:116-119 feeds it in training -- so one descriptor pass
+serves the whole K sweep.  The reference's save_keypoints.py computes no descriptors, so there is no reference policy for
+this.
 """
 import argparse
 import json
@@ -511,11 +517,11 @@ def main(argv=None):
     if a.descriptor_tree:
         ev.read_descriptor_tree(a.descriptor_tree, a.feature_dim)
     else:
-        from usip_b200.models.keypoint_descriptor import ModelDescriptor
+        from usip_b200.models.keypoint_descriptor import ModelDescriptorIndoor
         from usip_b200.models.keypoint_detector import ModelDetector
         from .registration import load_descriptor_checkpoint
         from .repeatability import load_detector_checkpoint
-        det, des = ModelDetector(opt), ModelDescriptor(opt)
+        det, des = ModelDetector(opt), ModelDescriptorIndoor(opt)
         load_detector_checkpoint(det, a.detector)
         load_descriptor_checkpoint(des, a.descriptor)
         ev.describe(det, des, a.nms_radius, L=ks[-1])

@@ -1,8 +1,12 @@
 """`ModelDescriptor` -- API surface of models/keypoint_descriptor.py:14-318 (outdoor descriptor: DescriptorLiteOld +
 DescPairScanLoss) on the fused H100 plan: `forward`, `forward_siamese`, `run_model`, `test_model` and the train step
 `optimize()` (backward plan in engine.descriptor_backward, loss backward in losses._DescTripletFn; SURVEY.md 8 f-1).
-`ModelDescriptorIndoor` depends on a network that is
-broken in the reference itself (networks.py:447 calls a commented-out function) and is out of scope."""
+
+`ModelDescriptorIndoor` -- models/keypoint_descriptor.py:321-600 (indoor descriptor: DescriptorLiteOldGlobal, 448-sample
+balls and a global context) -- runs forward only: `set_input`, `forward`, `forward_siamese`, `run_model` and
+`freeze_model`.  Its training (DescCGFLoss, `optimize`, `test_model`) is not implemented.  The reference network calls
+operations.ball_query_wrapper, which the reference ships commented out (operations.py:295-366); this plan follows that
+commented-out code, whose semantics are those of the reference's ball_query extension."""
 import os
 from collections import OrderedDict
 
@@ -149,3 +153,66 @@ class ModelDescriptor():
             g['lr'] = lr
         print('update descriptor learning rate: %f -> %f' % (self.old_lr_descriptor, lr))
         self.old_lr_descriptor = lr
+
+
+class ModelDescriptorIndoor():
+    """models/keypoint_descriptor.py:321-600 without its training: DescriptorLiteOldGlobal on the fused plan."""
+
+    def __init__(self, opt):
+        self.opt = opt
+        if opt.gpu_ids[0] < 0:
+            raise RuntimeError("usip_b200.ModelDescriptorIndoor needs a CUDA device: there is no CPU path")
+        self.descriptor = networks.DescriptorLiteOldGlobal(opt).to(opt.device)
+        self.old_lr_descriptor = self.opt.lr
+        dev = opt.device
+        B, N, M = opt.batch_size, opt.input_pc_num, opt.node_num
+        self.anc_pc = torch.empty(B, 3, N, device=dev).uniform_(); self.anc_sn = torch.empty(B, 3, N, device=dev).uniform_()
+        self.anc_keypoints = torch.empty(B, 3, M, device=dev); self.anc_sigmas = torch.empty(B, M, device=dev)
+        self.pos_pc = torch.empty(B, 3, N, device=dev).uniform_(); self.pos_sn = torch.empty(B, 3, N, device=dev).uniform_()
+        self.pos_keypoints = torch.empty(B, 3, M, device=dev); self.pos_sigmas = torch.empty(B, M, device=dev)
+        self.anc_R_pos = torch.zeros((B, 3, 3), dtype=torch.float32, device=dev)
+        self.anc_scale_pos = torch.zeros((B, 1), dtype=torch.float32, device=dev)
+        self.anc_shift_pos = torch.zeros((B, 3, 1), dtype=torch.float32, device=dev)
+
+    def set_input(self, anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas,
+                  anc_R_pos, anc_scale_pos, anc_shift_pos):
+        """keypoint_descriptor.py:369-389."""
+        dev = self.opt.device
+        self.anc_pc = anc_pc.float().to(dev); self.anc_sn = anc_sn.float().to(dev)
+        self.anc_keypoints = anc_keypoints.float().to(dev); self.anc_sigmas = anc_sigmas.float().to(dev)
+        self.pos_pc = pos_pc.float().to(dev); self.pos_sn = pos_sn.float().to(dev)
+        self.pos_keypoints = pos_keypoints.float().to(dev); self.pos_sigmas = pos_sigmas.float().to(dev)
+        self.anc_R_pos = anc_R_pos.float().to(dev); self.anc_scale_pos = anc_scale_pos.float().to(dev)
+        self.anc_shift_pos = anc_shift_pos.float().to(dev)
+        torch.cuda.synchronize()
+
+    def forward(self, pc, sn, keypoints, is_train=False, epoch=None):
+        with torch.cuda.device(pc.get_device()):
+            return self.descriptor(pc, sn, keypoints, is_train, epoch)
+
+    def forward_siamese(self, pc_tuple, sn_tuple, keypoints_tuple, is_train=False, epoch=None):
+        n = pc_tuple[0].size()[0]
+        descriptors, x_aug_ball = self.descriptor(torch.cat(pc_tuple, dim=0), torch.cat(sn_tuple, dim=0),
+                                                  torch.cat(keypoints_tuple, dim=0), is_train, epoch)
+        return torch.split(descriptors, n, dim=0), torch.split(x_aug_ball, n, dim=0)
+
+    def optimize(self, epoch=None):
+        raise NotImplementedError("ModelDescriptorIndoor.optimize needs DescCGFLoss and the descriptor's backward, which "
+                                  "are not implemented (forward and run_model are)")
+
+    def test_model(self):
+        raise NotImplementedError("ModelDescriptorIndoor.test_model needs DescCGFLoss, which is not implemented "
+                                  "(forward and run_model are)")
+
+    def freeze_model(self):
+        for p in self.descriptor.parameters():
+            p.requires_grad = False
+
+    def run_model(self, pc, sn, keypoints):
+        self.descriptor.eval()
+        with torch.cuda.device(pc.device), torch.no_grad():
+            descriptors, _ = self.descriptor(pc, sn, keypoints, False, None)
+        return descriptors
+
+    def save_network(self, network, network_label, epoch_label, gpu_id):
+        torch.save(network.state_dict(), os.path.join(self.opt.checkpoints_dir, '%s_net_%s.pth' % (epoch_label, network_label)))

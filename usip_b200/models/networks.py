@@ -5,6 +5,7 @@ in usip_b200/engine.py.
   RPN_Detector      models/networks.py:20-162   (C1=128, C2=512)
   RPN_DetectorLite  models/networks.py:165-307  (C1=64,  C2=256; same graph)
   DescriptorLiteOld models/networks.py:310-385
+  DescriptorLiteOldGlobal models/networks.py:388-479  (indoor: PPFNet global context; forward only)
   RPN_Detector_KNN  models/networks.py:482-608  (ablation: 64 nearest points per node instead of the SOM assignment)
   RPN_Detector_Ball models/networks.py:611-738  (ablation: first 64 points within radius 2 of each node)
 """
@@ -21,6 +22,16 @@ def _check_group(k, name):
     if k % 4 != 0 or 128 % k != 0:
         raise NotImplementedError("%s=%d: the H100 plan supports group sizes 4, 8, 16, 32, 64, 128 "
                                   "(every shipped configuration uses 16, 32 or 64)" % (name, k))
+
+
+def _check_ball(k, name):
+    """Balls of at most 128 rows go through the layer epilogue's group max directly; larger ones as 64-row sub-groups that
+    usip_group_max_combine reduces (engine._group_net_forward)."""
+    if k > 128 and k % 64 == 0:
+        return
+    if k % 4 != 0 or 128 % k != 0:
+        raise NotImplementedError("%s=%d: the H100 plan supports balls of 4, 8, 16, 32, 64 or 128 samples, or a multiple "
+                                  "of 64 above 128 (the indoor options use 448)" % (name, k))
 
 
 class _PackedWeightHooks:
@@ -241,3 +252,47 @@ class DescriptorLiteOld(_PackedWeightHooks, nn.Module):
         with torch.cuda.device(x.device):
             desc, feats = _DescriptorFn.apply(self, x, sn, keypoints, epoch, permute_idx, *params)
         return desc, feats
+
+
+class DescriptorLiteOldGlobal(_PackedWeightHooks, nn.Module):
+    """models/networks.py:388-479, the indoor descriptor: DescriptorLiteOld's grouped PointNet, then PPFNet's global
+    context -- the max of the descriptors over the M keypoints of each cloud, concatenated to every keypoint's descriptor,
+    fc1 (2D->2D), fc2 (2D->D), fc3 (D->D, linear) -- and L2 normalisation.  The global context is taken over the keypoints
+    the forward is given.  forward(x, sn, keypoints, is_train, epoch) -> (descriptor (B,D,M), x_features (B,3+S,M,K)).
+    Forward only: training (DescCGFLoss and its backward) is not implemented."""
+
+    def __init__(self, opt):
+        super().__init__()
+        self.opt = opt
+        cin = 3 + opt.surface_normal_len
+        D = int(opt.descriptor_len)                           # the indoor options declare descriptor_len as a float
+        bn = dict(momentum=opt.bn_momentum, bn_momentum_decay_step=opt.bn_momentum_decay_step,
+                  bn_momentum_decay=opt.bn_momentum_decay)
+        kw = dict(kernel_size=(1, 1), stride=1, padding=0, bias=True, activation=opt.activation,
+                  normalization=opt.normalization, **bn)
+        self.conv1 = MyConv2d(cin, D // 4, **kw)
+        self.conv2 = MyConv2d(D // 4, D // 2, **kw)
+        self.conv3 = MyConv2d(D // 2, D, **kw)
+        self.conv4 = MyConv2d(D * 2, D, **kw)
+        self.conv5 = MyConv2d(D, D, kernel_size=(1, 1), stride=1, padding=0, bias=True, activation=None, normalization=None)
+        self.fc1 = EquivariantLayer(D * 2, D * 2, activation=opt.activation, normalization=opt.normalization, **bn)
+        self.fc2 = EquivariantLayer(D * 2, D, activation=opt.activation, normalization=opt.normalization, **bn)
+        self.fc3 = EquivariantLayer(D, D, activation=None, normalization=None)
+        _check_ball(opt.ball_nsamples, "ball_nsamples")
+        if opt.activation != "relu" or opt.normalization != "batch":
+            raise NotImplementedError("the H100 plan implements activation='relu', normalization='batch'")
+        self.use_tc = bool(getattr(opt, "use_tensor_cores", True))
+        self._install_weight_hooks()
+
+    def forward(self, x, sn, keypoints, is_train=False, epoch=None):
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("DescriptorLiteOldGlobal runs forward only: training the indoor descriptor "
+                                      "(DescCGFLoss and its backward) is a follow-up.  Call it under torch.no_grad() or "
+                                      "freeze its parameters")
+        if not x.is_cuda:
+            raise RuntimeError("usip_b200 runs on CUDA tensors only (no CPU fallback)")
+        N = x.size()[2]
+        # host-side permutation, same RNG stream as the reference (networks.py:443)
+        permute_idx = torch.from_numpy(np.random.permutation(N).astype(np.int64)).to(x.device)
+        with torch.cuda.device(x.device):
+            return engine.descriptor_global_forward(self, x, sn, keypoints, epoch, permute_idx, use_tc=self.use_tc)

@@ -613,6 +613,24 @@ def group_select(gmax, gmin, scale, shift, out, Q, C):
                                         _stream()), "usip_group_select")
 
 
+def group_max_combine(gmax, ratio, gmin=None):
+    """[Q*ratio, C] per-sub-group max (and min) -> [Q, C]: the max (min) over each run of `ratio` consecutive rows."""
+    _req(gmax, f32, "gmax")
+    if gmin is not None:
+        _req(gmin, f32, "gmin")
+        if gmin.shape != gmax.shape:
+            raise ValueError("gmin %s must have gmax's shape %s" % (tuple(gmin.shape), tuple(gmax.shape)))
+    R, C = gmax.shape
+    if ratio < 1 or R % ratio != 0:
+        raise ValueError("group_max_combine: ratio %d must divide the %d rows" % (ratio, R))
+    Q = R // ratio
+    omax = torch.empty((Q, C), dtype=f32, device=gmax.device)
+    omin = None if gmin is None else torch.empty((Q, C), dtype=f32, device=gmax.device)
+    check(_lib.load().usip_group_max_combine(_p(gmax), _p(gmin), _p(omax), _p(omin), int(ratio), Q, C, _stream()),
+          "usip_group_max_combine")
+    return omax, omin
+
+
 def head_finalize(out4, cluster_mean, lb, B, M):
     kp = torch.empty((B, 3, M), dtype=f32, device=out4.device)
     sig = torch.empty((B, M), dtype=f32, device=out4.device)
