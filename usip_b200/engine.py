@@ -491,6 +491,49 @@ class _Bwd:
     def colsum(self, G, out, P, C):
         self.check(self.lib.usip_colsum(ops._p(G), G.stride(0), ops._p(out), P, C, ops._stream()), "usip_colsum")
 
+    def conv_bwd(self, GY, layer, P, X, prev=None, norm=None, name="", in_name="", cols=None, grad_in=True):
+        """Backward of the conv1x1 `layer` (y = act(X) W^T + b over P rows) from GY [P, Cout], the gradient of its pre-BN
+        output (of its output when it has no BatchNorm).  X: the saved input, read through relu(bn(.)) with the BNState
+        `prev` of the layer that produced it, or raw when prev is None; cols: the slice of W's columns a concat half reads.
+        Accumulates the weight (and bias) gradient and returns the gradient of act(X) -- or, given the input layer's
+        BatchNorm `norm`, of that layer's pre-BN output (profile record "bn_bwd_<in_name>"); GY is consumed then, its buffer
+        released before bn_bwd allocates the next one.  grad_in=False (a plan's first layer): the weight gradient only."""
+        W, gW = _w2d(layer.conv.weight), self.g2d(layer.conv.weight)
+        if cols is not None:
+            W, gW = _cols(W, cols.start, cols.stop), gW[:, cols]
+        Cout, Cin = W.shape
+        self.wgrad(GY, X, gW, P, Cout, Cin, prev=prev, name="wgrad_" + name)
+        # a conv bias in front of a train-mode BatchNorm receives exactly zero gradient (BN removes the mean): it stays
+        # zero-initialised in self.grads
+        if getattr(layer, "norm", None) is None:
+            self.colsum(GY, self.grads[layer.conv.bias], P, Cout)
+        if not grad_in:
+            return None
+        G_in = self.dgrad(GY, W, P, name="dgrad_" + name)
+        if norm is None:
+            return G_in
+        GY.set_()                                   # frees GY's buffer even though the caller still holds the tensor
+        return self.bn_bwd(G_in, X, prev, norm, P, Cin, name="bn_bwd_" + in_name)
+
+    def max_concat_bwd(self, GY, layer, X, prev, grp, amax, dense, node, K, Q, name):
+        """Backward of a layer on cat(a, broadcast max over each group of K rows of a), a = relu(bn(X)) (layers.py:435,
+        networks.py:377): y = a W[:, dense]^T + (amax W[:, node]^T)[row / K] + b, from GY [Q*K, Cout], the gradient of
+        its pre-BN output, which is consumed.  grp / prev: the group max/min/arg and BNState of the layer that produced
+        X.  Returns the gradient [Q*K, Cin] of a, the max path scattered to each group's selected row (the ReLU mask is
+        applied by the bn_bwd that follows)."""
+        p, s = ops._p, ops._stream
+        Cout = GY.shape[1]
+        G_a = self.conv_bwd(GY, layer, Q * K, X, prev, cols=dense, name=name)
+        G_U = torch.empty((Q, Cout), dtype=f32, device=self.dev)
+        self.check(self.lib.usip_group_sum(p(GY), GY.stride(0), p(G_U), G_U.stride(0), K, Q, Cout, s()), "usip_group_sum")
+        GY.set_()                                   # frees GY's buffer even though the caller still holds the tensor
+        G_amax = self.conv_bwd(G_U, layer, Q, amax, cols=node, name=name + "_node")
+        Cin = G_amax.shape[1]
+        _, arg, _, _ = self.groupmax_select(G_amax, grp, prev, Q, Cin, False)
+        self.check(self.lib.usip_groupmax_scatter_add(p(G_a), G_a.stride(0), p(G_amax), p(arg), K, Q, Cin, s()),
+                   "usip_groupmax_scatter_add")
+        return G_a
+
 
 def _knn_head_backward(bw, net, ctx, g_kp, g_sig):
     """Backward of _knn_head_forward: parameter gradients of mlp1/2/3 and knnlayer_1 are accumulated into bw.grads; returns
@@ -507,72 +550,33 @@ def _knn_head_backward(bw, net, ctx, g_kp, g_sig):
     # ---- head (networks.py:143-154)
     G_OUT = torch.empty((Q, 4), dtype=f32, device=dev)
     check(lib.usip_head_bwd(p(g_kp), p(g_sig), p(ctx["OUT"]), ctx["OUT"].stride(0), p(G_OUT), Bp, M, s()), "usip_head_bwd")
-    W12 = _w2d(net.mlp3.conv.weight)
-    bw.wgrad(G_OUT, ctx["Y11"], bw.g2d(net.mlp3.conv.weight), Q, 4, W12.shape[1], prev=ctx["bn11"], name="wgrad_mlp3")
-    bw.colsum(G_OUT, bw.grads[net.mlp3.conv.bias], Q, 4)
-    G_a11 = bw.dgrad(G_OUT, W12, Q, name="dgrad_mlp3")
-    GY11 = bw.bn_bwd(G_a11, ctx["Y11"], ctx["bn11"], net.mlp2.norm, Q, G_a11.shape[1])
-    W11 = _w2d(net.mlp2.conv.weight)
-    bw.wgrad(GY11, ctx["Y10"], bw.g2d(net.mlp2.conv.weight), Q, W11.shape[0], W11.shape[1], prev=ctx["bn10"], name="wgrad_mlp2")
-    G_a10 = bw.dgrad(GY11, W11, Q, name="dgrad_mlp2")
-    GY10 = bw.bn_bwd(G_a10, ctx["Y10"], ctx["bn10"], net.mlp1.norm, Q, G_a10.shape[1])
-    W10 = _w2d(net.mlp1.conv.weight)
-    bw.wgrad(GY10, ctx["AGG"], bw.g2d(net.mlp1.conv.weight), Q, W10.shape[0], W10.shape[1], name="wgrad_mlp1")
-    G_AGG = bw.dgrad(GY10, W10, Q, name="dgrad_mlp1")                      # [Q, C1+C2]
-    G_pool2 = G_AGG[:, :C1]
-    G_feat = G_AGG[:, C1:]
+    GY = bw.conv_bwd(G_OUT, net.mlp3, Q, ctx["Y11"], ctx["bn11"], net.mlp2.norm, "mlp3", "mlp2")
+    GY = bw.conv_bwd(GY, net.mlp2, Q, ctx["Y10"], ctx["bn10"], net.mlp1.norm, "mlp2", "mlp1")
+    G_AGG = bw.conv_bwd(GY, net.mlp1, Q, ctx["AGG"], name="mlp1")          # [Q, C1+C2]
 
-    # ---- kNN fusion, layers_after (layers.py:435-438)
-    groupmax_select = bw.groupmax_select
+    # ---- kNN fusion, layers_after (layers.py:435-438), last -> first
     Ya_last, bna_last = ctx["after"][-1]
-    GYa = bw.groupmax_bn_bwd(G_feat, Ya_last, ctx["grp_a"], bna_last, ka[-1].norm, Kn, Q, C2)
-    # remaining after-layers, last -> first (li >= 1: plain BN+ReLU chains)
+    GY = bw.groupmax_bn_bwd(G_AGG[:, C1:], Ya_last, ctx["grp_a"], bna_last, ka[-1].norm, Kn, Q, C2)
     for li in range(len(ka) - 1, 0, -1):
-        Wl = _w2d(ka[li].conv.weight)
-        Yin, bnin = ctx["after"][li - 1]
-        bw.wgrad(GYa, Yin, bw.g2d(ka[li].conv.weight), G, Wl.shape[0], Wl.shape[1], prev=bnin, name="wgrad_knn_a%d" % li)
-        G_in = bw.dgrad(GYa, Wl, G, name="dgrad_knn_a%d" % li)
-        GYa = bw.bn_bwd(G_in, Yin, bnin, ka[li - 1].norm, G, G_in.shape[1], name="bn_bwd_knn_a%d" % (li - 1))
-        del G_in
-    # ka[0]: Y8 = a7 Wnb^T + U[row/K] + b, U = amax Wmax^T
-    W8 = _w2d(ka[0].conv.weight)
+        GY = bw.conv_bwd(GY, ka[li], G, *ctx["after"][li - 1], ka[li - 1].norm, "knn_a%d" % li, "knn_a%d" % (li - 1))
+    # ka[0] on cat(broadcast max, a7): the max half is first
     Yb_last, bnb_last = ctx["before"][-1]
-    gW8 = bw.g2d(ka[0].conv.weight)
-    bw.wgrad(GYa, Yb_last, gW8[:, Cb:], G, C2, Cb, prev=bnb_last, name="wgrad_knn_a0")
-    G_a7 = bw.dgrad(GYa, _cols(W8, Cb), G, name="dgrad_knn_a0")               # [G, Cb]
-    G_U = torch.empty((Q, C2), dtype=f32, device=dev)
-    check(lib.usip_group_sum(p(GYa), GYa.stride(0), p(G_U), G_U.stride(0), Kn, Q, C2, s()), "usip_group_sum")
-    del GYa
-    bw.wgrad(G_U, ctx["amax"], gW8[:, :Cb], Q, C2, Cb, name="wgrad_knn_a0_node")
-    G_amax = bw.dgrad(G_U, _cols(W8, 0, Cb), Q, name="dgrad_knn_a0_node")        # [Q, Cb]
-    # max path joins the dense gradient of a7 at the arg rows (ReLU mask is applied by bn_bwd below)
-    _, arg7, _, _ = groupmax_select(G_amax, ctx["grp_b"], bnb_last, Q, Cb, False)
-    check(lib.usip_groupmax_scatter_add(p(G_a7), G_a7.stride(0), p(G_amax), p(arg7), Kn, Q, Cb, s()), "usip_groupmax_scatter_add")
+    GY = bw.max_concat_bwd(GY, ka[0], Yb_last, bnb_last, ctx["grp_b"], ctx["amax"], slice(Cb, None), slice(0, Cb), Kn, Q,
+                           "knn_a0")
     # ---- layers_before, last -> 1
-    GYb = bw.bn_bwd(G_a7, Yb_last, bnb_last, kb[-1].norm, G, Cb, name="bn_bwd_knn_b%d" % (len(kb) - 1))
-    del G_a7
+    GY = bw.bn_bwd(GY, Yb_last, bnb_last, kb[-1].norm, G, Cb, name="bn_bwd_knn_b%d" % (len(kb) - 1))
     for li in range(len(kb) - 1, 0, -1):
-        Wl = _w2d(kb[li].conv.weight)
-        Yin, bnin = ctx["before"][li - 1]
-        bw.wgrad(GYb, Yin, bw.g2d(kb[li].conv.weight), G, Wl.shape[0], Wl.shape[1], prev=bnin, name="wgrad_knn_b%d" % li)
-        G_in = bw.dgrad(GYb, Wl, G, name="dgrad_knn_b%d" % li)
-        GYb = bw.bn_bwd(G_in, Yin, bnin, kb[li - 1].norm, G, G_in.shape[1], name="bn_bwd_knn_b%d" % (li - 1))
-        del G_in
+        GY = bw.conv_bwd(GY, kb[li], G, *ctx["before"][li - 1], kb[li - 1].norm, "knn_b%d" % li, "knn_b%d" % (li - 1))
     # kb[0] = knn_combine: Y5 = Z[nbr] + Wxyz*delta + b, Z = pool2 Wf^T
-    W5 = _w2d(kb[0].conv.weight)
     gW5 = bw.g2d(kb[0].conv.weight)
     G_Z = torch.zeros((Q, Cb), dtype=f32, device=dev)
     with _Prof("knn_combine_bwd"):
-        check(lib.usip_knn_combine_bwd(p(GYb), GYb.stride(0), p(ctx["coords"]), p(ctx["knn_i"]), p(G_Z), G_Z.stride(0), p(gW5),
+        check(lib.usip_knn_combine_bwd(p(GY), GY.stride(0), p(ctx["coords"]), p(ctx["knn_i"]), p(G_Z), G_Z.stride(0), p(gW5),
                                        gW5.stride(0), Bp, M, Kn, Cb, s()), "usip_knn_combine_bwd")
-    del GYb
-    pool2 = ctx["AGG"][:, :C1]
-    bw.wgrad(G_Z, pool2, gW5[:, 3:], Q, Cb, C1, name="wgrad_knn_b0_node")
-    G_pool2_knn = bw.dgrad(G_Z, _cols(W5, 3), Q, name="dgrad_knn_b0_node")    # [Q, C1]
-    G_pool2_tot = G_pool2_knn
-    G_pool2_tot += G_pool2                                                 # tiny [Q,C1] plumbing add
-
-    return G_pool2_tot
+    del GY
+    G_pool2 = bw.conv_bwd(G_Z, kb[0], Q, ctx["AGG"][:, :C1], cols=slice(3, None), name="knn_b0_node")     # [Q, C1]
+    G_pool2 += G_AGG[:, :C1]                                               # tiny [Q,C1] plumbing add
+    return G_pool2
 
 
 def detector_backward(net, ctx, g_kp, g_sig):
@@ -585,48 +589,25 @@ def detector_backward(net, ctx, g_kp, g_sig):
     lib, check, p, s = bw.lib, bw.check, ops._p, ops._stream
     fp, sp = net.first_pointnet.layers, net.second_pointnet.layers
 
-    G_pool2_tot = _knn_head_backward(bw, net, ctx, g_kp, g_sig)
+    G_pool2 = _knn_head_backward(bw, net, ctx, g_kp, g_sig)
 
     # ---- pool 2 un-pool (index_max gather backward), second PointNet
     G_F2 = torch.zeros((P, C1), dtype=f32, device=dev)
-    check(lib.usip_unpool_scatter(p(G_F2), G_F2.stride(0), p(G_pool2_tot), G_pool2_tot.stride(0), p(ctx["arg2"]), Q, C1, 0, s()),
+    check(lib.usip_unpool_scatter(p(G_F2), G_F2.stride(0), p(G_pool2), G_pool2.stride(0), p(ctx["arg2"]), Q, C1, 0, s()),
           "usip_unpool_scatter")
-    W4 = _w2d(sp[1].conv.weight)
-    bw.wgrad(G_F2, ctx["Y3"], bw.g2d(sp[1].conv.weight), P, C1, C1, prev=ctx["bn3"], name="wgrad_pn2.1")
-    bw.colsum(G_F2, bw.grads[sp[1].conv.bias], P, C1)
-    G_a3 = bw.dgrad(G_F2, W4, P, name="dgrad_pn2.1")
-    del G_F2
-    GY3 = bw.bn_bwd(G_a3, ctx["Y3"], ctx["bn3"], sp[0].norm, P, C1, name="bn_bwd_pn2.0")
-    del G_a3
-    W3 = _w2d(sp[0].conv.weight)
-    gW3 = bw.g2d(sp[0].conv.weight)
-    bw.wgrad(GY3, ctx["F1"], gW3[:, :H], P, C1, H, name="wgrad_pn2.0")
-    G_F1 = bw.dgrad(GY3, _cols(W3, 0, H), P, name="dgrad_pn2.0")                  # [P, H]
+    GY3 = bw.conv_bwd(G_F2, sp[1], P, ctx["Y3"], ctx["bn3"], sp[0].norm, "pn2.1", "pn2.0")
+    # pn2.0 on cat(F1, un-pooled pool1): the per-node half's gradient is the segment sum
+    G_F1 = bw.conv_bwd(GY3, sp[0], P, ctx["F1"], cols=slice(0, H), name="pn2.0")                     # [P, H]
     G_V = torch.empty((Q, C1), dtype=f32, device=dev)
     check(lib.usip_seg_sum(p(GY3), GY3.stride(0), p(ctx["seg_off"]), p(G_V), G_V.stride(0), Bp, N, M, C1, s()), "usip_seg_sum")
     del GY3
-    bw.wgrad(G_V, ctx["pool1"], gW3[:, H:], Q, C1, H, name="wgrad_pn2.0_node")
-    G_pool1 = bw.dgrad(G_V, _cols(W3, H), Q, name="dgrad_pn2.0_node")          # [Q, H]
+    G_pool1 = bw.conv_bwd(G_V, sp[0], Q, ctx["pool1"], cols=slice(H, None), name="pn2.0_node")     # [Q, H]
     check(lib.usip_unpool_scatter(p(G_F1), G_F1.stride(0), p(G_pool1), G_pool1.stride(0), p(ctx["arg1"]), Q, H, 1, s()),
           "usip_unpool_scatter")
     # ---- first PointNet
-    W2 = _w2d(fp[2].conv.weight)
-    bw.wgrad(G_F1, ctx["Y1"], bw.g2d(fp[2].conv.weight), P, H, H, prev=ctx["bn1"], name="wgrad_pn1.2")
-    bw.colsum(G_F1, bw.grads[fp[2].conv.bias], P, H)
-    G_a1 = bw.dgrad(G_F1, W2, P, name="dgrad_pn1.2")
-    del G_F1
-    GY1 = bw.bn_bwd(G_a1, ctx["Y1"], ctx["bn1"], fp[1].norm, P, H, name="bn_bwd_pn1.1")
-    del G_a1
-    W1 = _w2d(fp[1].conv.weight)
-    bw.wgrad(GY1, ctx["Y0"], bw.g2d(fp[1].conv.weight), P, H, H, prev=ctx["bn0"], name="wgrad_pn1.1")
-    G_a0 = bw.dgrad(GY1, W1, P, name="dgrad_pn1.1")
-    del GY1
-    GY0 = bw.bn_bwd(G_a0, ctx["Y0"], ctx["bn0"], fp[0].norm, P, H, name="bn_bwd_pn1.0")
-    del G_a0
-    W0 = _w2d(fp[0].conv.weight)
-    bw.wgrad(GY0, ctx["X0"], bw.g2d(fp[0].conv.weight), P, H, W0.shape[1], name="wgrad_pn1.0")
-    # conv biases in front of a train-mode BatchNorm receive exactly zero gradient (BN removes the mean); they
-    # stay zero-initialised in bw.grads.
+    GY = bw.conv_bwd(G_F1, fp[2], P, ctx["Y1"], ctx["bn1"], fp[1].norm, "pn1.2", "pn1.1")
+    GY = bw.conv_bwd(GY, fp[1], P, ctx["Y0"], ctx["bn0"], fp[0].norm, "pn1.1", "pn1.0")
+    bw.conv_bwd(GY, fp[0], P, ctx["X0"], name="pn1.0", grad_in=False)
     return bw.result(net)
 
 
@@ -805,58 +786,19 @@ def descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=
 
 
 def _group_net_backward(bw, net, ctx, GY5):
-    """Backward of _group_net_forward from GY5 [G, C5], the gradient of conv5's raw output rows (parameter gradients are
-    accumulated into bw.grads; points / centres carry no gradient)."""
-    dev = bw.dev
+    """Backward of _group_net_forward from GY5 [G, C5], the gradient of conv5's raw output rows, which is consumed
+    (parameter gradients are accumulated into bw.grads; points / centres carry no gradient)."""
     Bp, M, K, D = ctx["Bp"], ctx["M"], ctx["K"], ctx["D"]
     Q, G = Bp * M, Bp * M * K
-    lib, check, p, s = bw.lib, bw.check, ops._p, ops._stream
     c1, c2, c3, c4, c5 = net.conv1, net.conv2, net.conv3, net.conv4, net.conv5
-    grp3 = ctx["grp3"]
-    C5 = c5.conv.weight.shape[0]
-    W5 = _w2d(c5.conv.weight)
-    bw.wgrad(GY5, ctx["Y4"], bw.g2d(c5.conv.weight), G, C5, W5.shape[1], prev=ctx["bn4"], name="wgrad_grp.conv5")
-    if getattr(c5, "norm", None) is None:
-        bw.colsum(GY5, bw.grads[c5.conv.bias], G, C5)          # a bias in front of a train-mode BN has exactly zero gradient
-    G_a4 = bw.dgrad(GY5, W5, G, name="dgrad_grp.conv5")
-    del GY5
-    GY4 = bw.bn_bwd(G_a4, ctx["Y4"], ctx["bn4"], c4.norm, G, G_a4.shape[1], name="bn_bwd_grp.conv4")
-    del G_a4
-    # ---- conv4 on cat(y_first, broadcast max): Y4 = a3 WA^T + U[row/K] + b,  U = amax WB^T
-    W4 = _w2d(c4.conv.weight)
-    gW4 = bw.g2d(c4.conv.weight)
-    C4 = W4.shape[0]
-    bw.wgrad(GY4, ctx["Y3"], gW4[:, :D], G, C4, D, prev=ctx["bn3"], name="wgrad_grp.conv4")
-    G_a3 = bw.dgrad(GY4, _cols(W4, 0, D), G, name="dgrad_grp.conv4")                 # [G, D]
-    G_U = torch.empty((Q, C4), dtype=f32, device=dev)
-    check(lib.usip_group_sum(p(GY4), GY4.stride(0), p(G_U), G_U.stride(0), K, Q, C4, s()), "usip_group_sum")
-    del GY4
-    bw.wgrad(G_U, ctx["amax"], gW4[:, D:], Q, C4, D, name="wgrad_grp.conv4_node")
-    G_amax = bw.dgrad(G_U, _cols(W4, D), Q, name="dgrad_grp.conv4_node")             # [Q, D]
-    # the max path joins the dense gradient of a3 at the arg rows (the ReLU mask is applied by bn_bwd below)
-    gz = torch.empty((Q, D), dtype=f32, device=dev); arg3 = torch.empty((Q, D), dtype=i32, device=dev)
-    bn3 = ctx["bn3"]
-    check(lib.usip_groupmax_bwd_select(p(G_amax), G_amax.stride(0), p(grp3["gmax"]), p(grp3["gmin"]), p(grp3["amax"]),
-                                       p(grp3["amin"]), p(bn3.scale), p(bn3.shift), p(bn3.mean), p(bn3.invstd), p(gz), p(arg3),
-                                       None, Q, D, s()), "usip_groupmax_bwd_select")
-    check(lib.usip_groupmax_scatter_add(p(G_a3), G_a3.stride(0), p(G_amax), p(arg3), K, Q, D, s()), "usip_groupmax_scatter_add")
-    # ---- conv3, conv2, conv1
-    GY3 = bw.bn_bwd(G_a3, ctx["Y3"], bn3, c3.norm, G, D, name="bn_bwd_grp.conv3")
-    del G_a3
-    W3 = _w2d(c3.conv.weight)
-    bw.wgrad(GY3, ctx["Y2"], bw.g2d(c3.conv.weight), G, W3.shape[0], W3.shape[1], prev=ctx["bn2"], name="wgrad_grp.conv3")
-    G_a2 = bw.dgrad(GY3, W3, G, name="dgrad_grp.conv3")
-    del GY3
-    GY2 = bw.bn_bwd(G_a2, ctx["Y2"], ctx["bn2"], c2.norm, G, G_a2.shape[1], name="bn_bwd_grp.conv2")
-    del G_a2
-    W2 = _w2d(c2.conv.weight)
-    bw.wgrad(GY2, ctx["Y1"], bw.g2d(c2.conv.weight), G, W2.shape[0], W2.shape[1], prev=ctx["bn1"], name="wgrad_grp.conv2")
-    G_a1 = bw.dgrad(GY2, W2, G, name="dgrad_grp.conv2")
-    del GY2
-    GY1 = bw.bn_bwd(G_a1, ctx["Y1"], ctx["bn1"], c1.norm, G, G_a1.shape[1], name="bn_bwd_grp.conv1")
-    del G_a1
-    W1 = _w2d(c1.conv.weight)
-    bw.wgrad(GY1, ctx["rows"], bw.g2d(c1.conv.weight), G, W1.shape[0], W1.shape[1], name="wgrad_grp.conv1")
+    GY = bw.conv_bwd(GY5, c5, G, ctx["Y4"], ctx["bn4"], c4.norm, "grp.conv5", "grp.conv4")
+    # conv4 on cat(a3, broadcast max): the max half is last
+    GY = bw.max_concat_bwd(GY, c4, ctx["Y3"], ctx["bn3"], ctx["grp3"], ctx["amax"], slice(0, D), slice(D, None), K, Q,
+                           "grp.conv4")
+    GY = bw.bn_bwd(GY, ctx["Y3"], ctx["bn3"], c3.norm, G, D, name="bn_bwd_grp.conv3")
+    GY = bw.conv_bwd(GY, c3, G, ctx["Y2"], ctx["bn2"], c2.norm, "grp.conv3", "grp.conv2")
+    GY = bw.conv_bwd(GY, c2, G, ctx["Y1"], ctx["bn1"], c1.norm, "grp.conv2", "grp.conv1")
+    bw.conv_bwd(GY, c1, G, ctx["rows"], name="grp.conv1", grad_in=False)
 
 
 def descriptor_backward(net, ctx, g_desc):
