@@ -450,9 +450,19 @@ int usip_group_select(const float* gmax, const float* gmin, const float* scale, 
  * out_min likewise from gmin, when both are given) for Q_out x C outputs, rows contiguous ([Q_out*ratio, C] in,
  * [Q_out, C] out).  Same comparison as the epilogue's group max (strict >, strict <, from -inf / +inf; NaN never wins)
  * and the result of one in-order scan, so it is deterministic.  The indoor descriptor uses it for its 448-row balls
- * (64-row sub-groups, ratio 7) and for the per-cloud global max over its M keypoints (ratio M).  No arg outputs. */
+ * (64-row sub-groups, ratio 7) and for the per-cloud global max over its M keypoints (ratio M).  No arg outputs: see
+ * usip_group_max_combine_arg. */
 int usip_group_max_combine(const float* gmax, const float* gmin, float* out_max, float* out_min, int ratio, int Q_out,
                            int C, void* stream);
+/* The same combine with arg outputs, for the backward of the indoor descriptor.  out_amax [Q_out, C] i32 is the row of
+ * out_max in the whole group: r * sub + amax[q*ratio + r, c], where r < ratio is the first input row holding the max
+ * (row 0 when none beats -inf: all -inf / NaN) and amax the row-in-sub-group args of the layer epilogue; with amax NULL
+ * (the global max over keypoints) it is r.  out_amin likewise from gmin / amin.  With ties at the first index inside each
+ * sub-group, the arg is the first index of the max over all ratio * sub rows.  gmax, out_max, out_amax are required;
+ * gmin, out_min, out_amin come together; amin comes with amax (and gmin); sub >= 1 with args. */
+int usip_group_max_combine_arg(const float* gmax, const float* gmin, const int32_t* amax, const int32_t* amin,
+                               float* out_max, float* out_min, int32_t* out_amax, int32_t* out_amin, int ratio, int sub,
+                               int Q_out, int C, void* stream);
 
 /* networks.py:151-154: keypoints (B,3,M) = out[:, :3] + cluster_mean ; sigmas (B,M) = softplus(out[:,3]) + lb */
 int usip_head_finalize(const float* out4, int ld, const float* cluster_mean, float sigma_lower_bound,
@@ -506,6 +516,31 @@ int usip_desc_triplet_bwd(const float* anc, const float* pos, const float* neg, 
                           const float* dneg, const int32_t* ineg, const float* sigma, float gamma, float sigma_max,
                           const float* g_loss, float* g_anc, float* g_pos, float* g_neg, int B, int C, int M, int Mp,
                           int Mn, void* stream);
+/* DescCGFLoss (models/losses.py:240-369), the indoor descriptor's triplet loss, without its (B,M,M) and (B,C,M,M)
+ * intermediates.  anc_kp (B,3,M) already in the positive frame, pos_kp (B,3,M), anc_desc / pos_desc (B,D,M), sigma (B,M),
+ * the reference's three draws u_near, u_out (B,M,M) and u_sel (B,M), all contiguous.  For each anchor m, over the positive
+ * keypoints j (d = sqrt((dx*dx + dy*dy) + dz*dz) in fp32 without contraction, mask = d <= radius), first index on ties:
+ *   near = argmax (mask ? u_near : 0),  far = argmax -(d + (mask ? 1000 : 0)),  out = argmax (!mask ? u_out : 0)
+ * and only those three descriptor distances.  Per cloud (fixed-order sums): scaling = M / (count + 1),
+ * w = clamp(sigma_max - sigma, 0) / mean, neg = u_sel < 0.5 ? d_far : d_out,
+ * before_clamp = (d_near - neg + gamma) * mask, loss (B,M) = w * clamp(before_clamp, 0) * scaling,
+ * active (B) = #(before_clamp > 1e-5) / (count + 1).  Saved for the backward: sel (B,M,4) i32 = near, far, out, flags
+ * (bit 0 mask, bit 1 u_sel < 0.5), aux (B,M,4) f32 = d_near, d_far, d_out, before_clamp, cloud (B,2) f32 = scaling, mean
+ * weight; sel and aux 16-byte aligned.  Limits: M <= USIP_CGF_MAX_M (the positive keypoints are staged in shared
+ * memory), D a multiple of 4 in [4, USIP_CGF_MAX_D] (the backward keeps D/32 channels per lane in registers). */
+#define USIP_CGF_MAX_M 2048
+#define USIP_CGF_MAX_D 512
+int usip_desc_cgf_f32(const float* anc_kp, const float* pos_kp, const float* anc_desc, const float* pos_desc,
+                      const float* sigma, const float* u_near, const float* u_out, const float* u_sel, float radius,
+                      float gamma, float sigma_max, float* loss, float* active, int32_t* sel, float* aux, float* cloud,
+                      int B, int M, int D, void* stream);
+/* backward of usip_desc_cgf_f32 for the upstream gradient g_loss (B,M): g_anc, g_pos (B,D,M) OVERWRITTEN.  Per anchor,
+ * coef = ((g * scaling) * w) * [before_clamp >= 0] * mask (torch's clamp passes the gradient at 0); the pairs near, far,
+ * out receive coef, -coef * [u_sel < 0.5], -coef * [u_sel >= 0.5] times (a - p) / d, exactly 0 where d == 0.  g_pos is
+ * gathered positive-major (each positive keypoint walks the anchors in order): bit-reproducible, no atomics. */
+int usip_desc_cgf_bwd(const float* anc_desc, const float* pos_desc, const float* sigma, const int32_t* sel,
+                      const float* aux, const float* cloud, const float* g_loss, float sigma_max, float* g_anc,
+                      float* g_pos, int B, int M, int D, void* stream);
 /* backward of usip_l2norm_to_bcm: g (B,C,M), raw rows Y [B*M, C] -> GY [B*M, C]                     networks.py:383 */
 int usip_l2norm_bwd(const float* g, const float* Y, int ldy, float* GY, int ldg, int B, int M, int C, void* stream);
 

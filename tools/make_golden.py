@@ -243,6 +243,81 @@ def golden_descriptor_train(ref):
     print("descriptor train loss", out["loss"], "active", out["active"])
 
 
+INDOOR_TRAIN = dict(B=2, N=2048, M=64, S=4, K=448, D=128, seed=91, radius=0.75, cgf_radius=0.075, gamma=0.3, sigma_max=0.5)
+
+
+def golden_descriptor_indoor_train(ref):
+    """One ModelDescriptorIndoor.optimize() and one test_model() of the reference (keypoint_descriptor.py:451-519) on the
+    CPU, with tests/desc_indoor_ref.py supplying ball_query_wrapper: the three torch.rand draws of each DescCGFLoss call,
+    the picks (the index arguments of its three torch.gather calls), per-anchor loss and active share, the descriptors,
+    gradient and post-Adam parameter summaries (descriptor_train.npz's format).  Inputs: tests/cgf_ref.train_inputs."""
+    from tests import cgf_ref
+    from tests import desc_indoor_ref as dref
+    c = INDOOR_TRAIN
+    B, N, M, S, K, D, seed = (c[k] for k in ("B", "N", "M", "S", "K", "D", "seed"))
+    d = cgf_ref.train_inputs(B, N, M, S, seed, radius=c["cgf_radius"])
+    dref.install(ref)
+    opt = ref_shim.make_opt(batch_size=B, input_pc_num=N, node_num=M, surface_normal_len=S, ball_radius=c["radius"],
+                            ball_nsamples=K, descriptor_len=D, random_pc_dropout_lower_limit=1.0,
+                            CGF_radius=c["cgf_radius"], triple_loss_gamma=c["gamma"], sigma_max=c["sigma_max"])
+    torch.manual_seed(seed); np.random.seed(seed); random.seed(seed)
+    md = ref.keypoint_descriptor.ModelDescriptorIndoor(opt)
+    out = dict(cfg=np.array([B, N, M, S, K, D, seed], np.int64),
+               radii=np.array([c["radius"], c["cgf_radius"], c["gamma"], c["sigma_max"]], np.float64))
+    for k, v in md.descriptor.state_dict().items():
+        out["param/" + k] = v.detach().numpy().copy()
+    md.set_input(*[t(d[k]) for k in cgf_ref.SET_INPUT_KEYS])
+    crit = md.triplet_criteria.forward
+
+    def recording(tag):
+        def forward(*a, **k):
+            draws, picks = [], []
+            rand, gather = torch.rand, torch.gather
+
+            def rec_rand(*ra, **rk):
+                draws.append(rand(*ra, **rk)); return draws[-1]
+
+            def rec_gather(x, dim, index, *ga, **gk):
+                picks.append(index.squeeze(2)); return gather(x, dim, index, *ga, **gk)
+            torch.rand, torch.gather = rec_rand, rec_gather
+            try:
+                loss, active = crit(*a, **k)
+            finally:
+                torch.rand, torch.gather = rand, gather
+            assert len(draws) == 3 and len(picks) == 3
+            for name, v in zip(("u_near", "u_out", "u_sel"), draws):
+                out["%s/%s" % (tag, name)] = v.numpy()
+            for name, v in zip(("near", "far", "out"), picks):
+                out["%s/%s" % (tag, name)] = v.numpy().astype(np.int16)
+            out[tag + "/anc_kp_t"] = a[0].detach().numpy()
+            out[tag + "/loss_vec"] = loss.detach().numpy(); out[tag + "/active_vec"] = active.detach().numpy()
+            return loss, active
+        return forward
+    md.triplet_criteria.forward = recording("train")
+    np.random.seed(seed)                                   # the forward consumes np.random.permutation(N)
+    md.optimize(epoch=0)
+    out["loss"] = np.float32(md.loss.item()); out["active"] = np.float32(md.active_percentage.item())
+    out["anc_desc"] = md.anc_descriptors.detach().numpy(); out["pos_desc"] = md.pos_descriptors.detach().numpy()
+    for k, p in md.descriptor.named_parameters():
+        g = p.grad.detach().numpy().reshape(-1).astype(np.float64)
+        out["grad/" + k] = np.concatenate([[g.mean(), g.std(), np.abs(g).max(), np.linalg.norm(g)], g[:24]]).astype(np.float32)
+    for k, v in md.descriptor.state_dict().items():
+        v = v.detach().numpy()
+        if k.endswith("num_batches_tracked"):
+            continue
+        flat = v.reshape(-1).astype(np.float64)
+        out["after/" + k] = np.concatenate([[flat.mean(), flat.std(), np.abs(flat).max()], flat[:24]]).astype(np.float32)
+    md.triplet_criteria.forward = recording("test")
+    np.random.seed(seed + 1)
+    md.test_model()
+    out["test_loss"] = np.float32(md.loss.item()); out["test_active"] = np.float32(md.active_percentage.item())
+    print("descriptor_indoor_train: loss %.6f active %.4f, test loss %.6f, anchors with a positive %d of %d" % (
+        out["loss"], out["active"], out["test_loss"], int(cgf_ref.selections(
+            t(out["train/anc_kp_t"]), t(d["pos_kp"]), t(out["train/u_near"]), t(out["train/u_out"]),
+            c["cgf_radius"])[3].sum()), B * M))
+    np.savez_compressed(os.path.join(OUT, "descriptor_indoor_train.npz"), **out)
+
+
 def desc_train_inputs(B, N, M, S, seed):
     """Synthetic (anchor, positive) scan pair with keypoints + sigmas for the descriptor train step (shared with the
     tests through oracle.usip_oracle.desc_train_inputs)."""
@@ -844,6 +919,7 @@ def main():
     golden_desc_loss(ref)
     golden_descriptor_train(ref)
     golden_descriptor_indoor(ref)
+    golden_descriptor_indoor_train(ref)
     golden_fps(ref)
     golden_nms(ref)
     golden_ablation(ref)

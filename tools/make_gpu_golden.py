@@ -137,6 +137,76 @@ def descriptor_indoor_golden(ref, out):
     np.savez_compressed(os.path.join(out, "reference_descriptor_indoor.npz"), **g)
 
 
+def descriptor_indoor_train_golden(ref, out):
+    """One ModelDescriptorIndoor.optimize() of the reference at SceneNN's training shape (B=2 pairs, N=5000, M=512, K=448,
+    D=128, radius 0.75, CGF_radius 0.075, gamma 0.3, sigma_max 0.5) after torch.cuda.manual_seed, in float32 and in
+    float64 (the same modules and draws): the picks (its three torch.gather indices), loss, active share, sampled float64
+    gradients, their scales and the float32 run's own error against them (DESIGN section 2)."""
+    from tests import cgf_ref
+    from tests import desc_indoor_ref as dref
+    from tests import test_gpu_descriptor_indoor_train as TI
+    c = TI.FULL
+    opt, d, state = TI.full_setup()
+    dref.install(ref)
+    ref_opt = ref_shim.make_opt(**{k: getattr(opt, k) for k in vars(opt) if k != "use_tensor_cores"})
+    runs = {}
+    for dtype in (torch.float32, torch.float64):
+        md = ref.keypoint_descriptor.ModelDescriptorIndoor(ref_opt)
+        md.descriptor.load_state_dict(state)
+        if dtype == torch.float64:
+            md.descriptor.double()
+            md.optimizer_descriptor = torch.optim.Adam(md.descriptor.parameters(), lr=ref_opt.lr, betas=(0.9, 0.999),
+                                                       weight_decay=0)
+        ins = [torch.from_numpy(d[k]) for k in cgf_ref.SET_INPUT_KEYS]
+        md.set_input(*ins)
+        if dtype == torch.float64:                           # set_input keeps float32 placeholders: cast the batch
+            for k in ("anc_pc", "anc_sn", "anc_keypoints", "anc_sigmas", "pos_pc", "pos_sn", "pos_keypoints", "pos_sigmas",
+                      "anc_R_pos", "anc_scale_pos", "anc_shift_pos"):
+                setattr(md, k, getattr(md, k).double())
+        picks = []
+        gather = torch.gather
+
+        def rec_gather(x, dim, index, *a, **k):
+            if index.dim() == 3 and index.shape[2] == 1 and x.shape[1] == x.shape[2]:
+                picks.append(index.squeeze(2).cpu().numpy())
+            return gather(x, dim, index, *a, **k)
+        bq = sys.modules["ball_query"].forward_cuda_shared_mem
+        sys.modules["ball_query"].forward_cuda_shared_mem = lambda dist, r, n: bq(dist.float().contiguous(), r, n)
+        torch.gather = rec_gather
+        try:
+            torch.cuda.manual_seed(c["seed"])
+            np.random.seed(c["seed"])
+            md.optimize(epoch=0)
+            torch.cuda.synchronize()
+        finally:
+            torch.gather = gather
+            sys.modules["ball_query"].forward_cuda_shared_mem = bq
+        assert len(picks) == 3, len(picks)
+        runs[dtype] = dict(picks=picks, loss=md.loss.item(), active=md.active_percentage.item(),
+                           grad={k: p.grad.detach().cpu().numpy().astype(np.float64)
+                                 for k, p in md.descriptor.named_parameters()})
+        del md
+        torch.cuda.empty_cache()
+    r32, r64 = runs[torch.float32], runs[torch.float64]
+    for a, b in zip(r32["picks"], r64["picks"]):
+        assert np.array_equal(a, b), "float32 and float64 runs picked differently"
+    g = dict(near=r32["picks"][0], far=r32["picks"][1], out=r32["picks"][2], loss32=np.float64(r32["loss"]),
+             loss64=np.float64(r64["loss"]), active=np.float32(r32["active"]))
+    for k, g64 in r64["grad"].items():
+        g32 = r32["grad"][k]
+        idx = TI.grad_sample(k, g64.size)
+        scale = np.abs(g64).max()
+        if k.endswith("conv.bias") and np.linalg.norm(g64) < 1e-6 * np.linalg.norm(r64["grad"][k.replace("bias", "weight")]):
+            scale = 0.0                                       # in front of a train-mode BatchNorm: true gradient 0
+        g["g64__" + k] = g64.ravel()[idx]
+        g["gscale__" + k] = np.float64(scale)
+        g["gnorm__" + k] = np.float64(np.linalg.norm(g64))
+        g["eref__" + k] = np.float64(np.abs(g32 - g64).max() / scale if scale else 0.0)
+    print("descriptor_indoor_train: loss fp32 %.7f fp64 %.7f, worst fp32 gradient error %.2e" % (
+        r32["loss"], r64["loss"], max(float(v) for k, v in g.items() if k.startswith("eref__"))))
+    np.savez_compressed(os.path.join(out, "reference_descriptor_indoor_train.npz"), **g)
+
+
 def main():
     out = sys.argv[1]
     only = sys.argv[2:]                        # e.g. `descriptor_indoor`: regenerate that file only
@@ -156,6 +226,7 @@ def main():
         detector_golden(ref, name, out)
     descriptor_golden(ref, out)
     descriptor_indoor_golden(ref, out)
+    descriptor_indoor_train_golden(ref, out)
     for f in sorted(os.listdir(out)):
         print(f, os.path.getsize(os.path.join(out, f)))
 

@@ -110,6 +110,7 @@ SIGNATURES = {
                                  c_int, c_int, c_int, c_int, c_ptr]),
     "usip_group_select": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_group_max_combine": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
+    "usip_group_max_combine_arg": (c_int, [c_ptr] * 8 + [c_int, c_int, c_int, c_int, c_ptr]),
     "usip_head_finalize": (c_int, [c_ptr, c_int, c_ptr, c_f32, c_ptr, c_ptr, c_int, c_int, c_ptr]),
     "usip_l2norm_to_bcm": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_pairwise_min_f32": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
@@ -122,6 +123,8 @@ SIGNATURES = {
     "usip_mean_scale": (c_int, [c_ptr, c_i64, c_f32, c_ptr, c_ptr]),
     "usip_desc_pairmin_f32": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_int, c_ptr]),
     "usip_desc_triplet": (c_int, [c_ptr, c_ptr, c_ptr, c_f32, c_f32, c_ptr, c_ptr, c_int, c_int, c_ptr]),
+    "usip_desc_cgf_f32": (c_int, [c_ptr] * 8 + [c_f32, c_f32, c_f32] + [c_ptr] * 5 + [c_int, c_int, c_int, c_ptr]),
+    "usip_desc_cgf_bwd": (c_int, [c_ptr] * 7 + [c_f32, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_pairwise_min_bwd": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_f32, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_chamfer_prob_bwd": (c_int, [c_ptr] * 13 + [c_int, c_int, c_int, c_ptr]),
     "usip_transform_points_bwd": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_ptr]),
@@ -177,7 +180,7 @@ def load():
 WEIGHT_GEN = [0]
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
-KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_cloud_subsample": 2, "usip_fragment_overlap_f32": 6}
+KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_cloud_subsample": 2, "usip_fragment_overlap_f32": 6, "usip_desc_cgf_f32": 2, "usip_desc_cgf_bwd": 2}
 LAUNCHES = [0]
 
 

@@ -344,6 +344,217 @@ desc_triplet_kernel(const float* __restrict__ dpos, const float* __restrict__ dn
 }
 
 
+// ---------------------------------------------------------------------------------------------------------------------
+// DescCGFLoss (models/losses.py:240-369) without its (B,M,M) distance matrices and (B,C,M,M) descriptor differences.
+// Anchor keypoints arrive already mapped into the positive frame.  Per anchor m of cloud b, over the M positive keypoints j
+// (d = ||a_m - p_j||, fp32 without contraction; mask = d <= radius):
+//   near = argmax_j (mask ? u_near[b,m,j] : 0)      far = argmin_j (d + (mask ? 1000 : 0))      out = argmax_j (!mask ? u_out : 0)
+// first index on ties (torch.max / torch.min along a dim), then the D-dimensional descriptor distances of those three
+// pairs only.  sel (B,M,4) int32 = near, far, out, flags (bit 0: the anchor has a positive, bit 1: u_sel < 0.5, the
+// negative is `far`); aux (B,M,4) f32 = the three descriptor distances and before_clamp; cloud (B,2) = scaling and the
+// sigma-weight mean, for the backward.
+constexpr int CGF_WARPS = 8;
+
+__global__ void __launch_bounds__(CGF_WARPS * 32)
+desc_cgf_select_kernel(const float* __restrict__ anc_kp, const float* __restrict__ pos_kp, const float* __restrict__ anc_desc,
+                       const float* __restrict__ pos_desc, const float* __restrict__ u_near, const float* __restrict__ u_out,
+                       const float* __restrict__ u_sel, float radius, float gamma, int32_t* __restrict__ sel,
+                       float* __restrict__ aux, int M, int D) {
+  __shared__ float sp[3][USIP_CGF_MAX_M];
+  const int b = blockIdx.y;
+  const float* pk = pos_kp + (size_t)b * 3 * M;
+  for (int t = threadIdx.x; t < 3 * M; t += blockDim.x) sp[t / M][t % M] = pk[t];
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int m = blockIdx.x * CGF_WARPS + (threadIdx.x >> 5);
+  if (m >= M) return;
+  const float* ak = anc_kp + (size_t)b * 3 * M;
+  const float ax = ak[m], ay = ak[M + m], az = ak[2 * M + m];
+  const float* un = u_near + ((size_t)b * M + m) * M;
+  const float* uo = u_out + ((size_t)b * M + m) * M;
+  float bn = -INFINITY, bf = INFINITY, bo = -INFINITY;
+  int jn = M, jf = M, jo = M, cnt = 0;
+  for (int j = lane; j < M; j += 32) {                  // each lane scans its columns in increasing j: strict compares
+    const float d = sqrtf(sqdist_rn(ax, ay, az, sp[0][j], sp[1][j], sp[2][j]));
+    const bool in = d <= radius;
+    const float vn = in ? __ldg(un + j) : 0.f;
+    const float vf = __fadd_rn(d, in ? 1000.f : 0.f);
+    const float vo = in ? 0.f : __ldg(uo + j);
+    if (vn > bn) { bn = vn; jn = j; }
+    if (vf < bf) { bf = vf; jf = j; }
+    if (vo > bo) { bo = vo; jo = j; }
+    cnt += in;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {                    // merge lanes: better value, then smaller index
+    const float xn = __shfl_xor_sync(0xffffffffu, bn, o), xf = __shfl_xor_sync(0xffffffffu, bf, o);
+    const float xo = __shfl_xor_sync(0xffffffffu, bo, o);
+    const int kn = __shfl_xor_sync(0xffffffffu, jn, o), kf = __shfl_xor_sync(0xffffffffu, jf, o);
+    const int ko = __shfl_xor_sync(0xffffffffu, jo, o);
+    if (xn > bn || (xn == bn && kn < jn)) { bn = xn; jn = kn; }
+    if (xf < bf || (xf == bf && kf < jf)) { bf = xf; jf = kf; }
+    if (xo > bo || (xo == bo && ko < jo)) { bo = xo; jo = ko; }
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  jn = jn < M ? jn : 0; jf = jf < M ? jf : 0; jo = jo < M ? jo : 0;
+  // descriptor distances of the three picks (lanes over channels, one fixed-order warp sum each)
+  const float* ad = anc_desc + (size_t)b * D * M;
+  const float* pd = pos_desc + (size_t)b * D * M;
+  float sn = 0.f, sf = 0.f, so = 0.f;
+  for (int c = lane; c < D; c += 32) {
+    const float a = ad[(size_t)c * M + m];
+    const float en = a - pd[(size_t)c * M + jn], ef = a - pd[(size_t)c * M + jf], eo = a - pd[(size_t)c * M + jo];
+    sn = fmaf(en, en, sn); sf = fmaf(ef, ef, sf); so = fmaf(eo, eo, so);
+  }
+  sn = warp_sum(sn); sf = warp_sum(sf); so = warp_sum(so);
+  if (lane == 0) {
+    const size_t t = (size_t)b * M + m;
+    const int flags = (cnt > 0 ? 1 : 0) | (u_sel[t] < 0.5f ? 2 : 0);
+    *reinterpret_cast<int4*>(sel + 4 * t) = make_int4(jn, jf, jo, flags);
+    const float dn = sqrtf(sn), df = sqrtf(sf), dout = sqrtf(so);
+    const float neg = (flags & 2) ? df : dout;
+    const float bc = __fmul_rn(__fadd_rn(__fsub_rn(dn, neg), gamma), (flags & 1) ? 1.f : 0.f);   // losses.py:318
+    *reinterpret_cast<float4*>(aux + 4 * t) = make_float4(dn, df, dout, bc);
+  }
+}
+
+// Per cloud, one CTA, fixed-order sums: scaling = M / (count + 1), w = clamp(sigma_max - sigma, 0) / mean_m(...),
+// loss = (w * clamp(before_clamp, 0)) * scaling, active = #(before_clamp > 1e-5) / (count + 1)      (losses.py:312-326).
+// A cloud whose sigmas are all >= sigma_max has mean 0 and NaN weights, as the reference.
+__global__ void __launch_bounds__(256)
+desc_cgf_reduce_kernel(const float* __restrict__ sigma, const int32_t* __restrict__ sel, const float* __restrict__ aux,
+                       float sigma_max, float* __restrict__ loss, float* __restrict__ active, float* __restrict__ cloud, int M) {
+  __shared__ double sh[32];
+  __shared__ float s_scale, s_wmean;
+  const int b = blockIdx.x;
+  double wsum = 0.0, cnt = 0.0, act = 0.0;
+  for (int m = threadIdx.x; m < M; m += 256) {
+    const size_t t = (size_t)b * M + m;
+    wsum += fmaxf(sigma_max - sigma[t], 0.f);
+    cnt += (sel[4 * t + 3] & 1) ? 1.0 : 0.0;
+    act += aux[4 * t + 3] > 1e-5f ? 1.0 : 0.0;
+  }
+  double r = block_sum(wsum, sh);
+  if (threadIdx.x == 0) s_wmean = (float)(r / M);
+  r = block_sum(cnt, sh);
+  const double a = block_sum(act, sh);
+  if (threadIdx.x == 0) {
+    const float den = (float)r + 1.f;
+    s_scale = (float)M / den;
+    active[b] = (float)a / den;
+    cloud[2 * b] = s_scale;
+    cloud[2 * b + 1] = s_wmean;
+  }
+  __syncthreads();
+  for (int m = threadIdx.x; m < M; m += 256) {
+    const size_t t = (size_t)b * M + m;
+    const float w = fmaxf(sigma_max - sigma[t], 0.f) / s_wmean;
+    const float bc = aux[4 * t + 3];
+    loss[t] = __fmul_rn(__fmul_rn(w, bc < 0.f ? 0.f : bc), s_scale);
+  }
+}
+
+// Coefficient of anchor t in the backward, torch's order through the graph of losses.py:318-326:
+// ((g * scaling) * w) * [before_clamp >= 0] * mask  (clamp passes the gradient at exactly 0).
+__device__ __forceinline__ float cgf_coef(const float* __restrict__ g, const float* __restrict__ sigma,
+                                          const float* __restrict__ cloud, const int32_t* __restrict__ sel,
+                                          const float* __restrict__ aux, float sigma_max, int b, size_t t) {
+  const float w = fmaxf(sigma_max - sigma[t], 0.f) / cloud[2 * b + 1];
+  const float c = __fmul_rn(__fmul_rn(g[t], cloud[2 * b]), w);
+  return __fmul_rn(__fmul_rn(c, aux[4 * t + 3] >= 0.f ? 1.f : 0.f), (sel[4 * t + 3] & 1) ? 1.f : 0.f);
+}
+
+// The three per-pair factors s_k of the norm backward, grad(d_k) / d_k and exactly 0 where d_k == 0 (torch's norm
+// backward): grad(near) = coef, grad(far) = -coef * sel, grad(out) = -coef * (1 - sel).
+__device__ __forceinline__ void cgf_pair_scales(float coef, int flags, float4 dd, float s[3]) {
+  const float f = (flags & 2) ? 1.f : 0.f;
+  const float gk[3] = {coef, -__fmul_rn(coef, f), -__fmul_rn(coef, 1.f - f)};
+  const float dk[3] = {dd.x, dd.y, dd.z};
+#pragma unroll
+  for (int k = 0; k < 3; ++k) s[k] = dk[k] == 0.f ? 0.f : gk[k] / dk[k];
+}
+
+// g_anc[b, :, m] = sum_k (a_m - p_{pick_k}) * s_k        (warp per anchor, lanes over channels)
+__global__ void __launch_bounds__(CGF_WARPS * 32)
+desc_cgf_bwd_anchor_kernel(const float* __restrict__ anc_desc, const float* __restrict__ pos_desc,
+                           const float* __restrict__ sigma, const int32_t* __restrict__ sel, const float* __restrict__ aux,
+                           const float* __restrict__ cloud, const float* __restrict__ g, float sigma_max,
+                           float* __restrict__ g_anc, int M, int D) {
+  const int b = blockIdx.y, lane = threadIdx.x & 31;
+  const int m = blockIdx.x * CGF_WARPS + (threadIdx.x >> 5);
+  if (m >= M) return;
+  const size_t t = (size_t)b * M + m;
+  const int4 pk = *reinterpret_cast<const int4*>(sel + 4 * t);
+  float s[3];
+  cgf_pair_scales(cgf_coef(g, sigma, cloud, sel, aux, sigma_max, b, t), pk.w,
+                  *reinterpret_cast<const float4*>(aux + 4 * t), s);
+  const float* ad = anc_desc + (size_t)b * D * M;
+  const float* pd = pos_desc + (size_t)b * D * M;
+  for (int c = lane; c < D; c += 32) {
+    const float a = ad[(size_t)c * M + m];
+    float v = (a - pd[(size_t)c * M + pk.x]) * s[0];
+    v += (a - pd[(size_t)c * M + pk.y]) * s[1];
+    v += (a - pd[(size_t)c * M + pk.z]) * s[2];
+    g_anc[(size_t)b * D * M + (size_t)c * M + m] = v;
+  }
+}
+
+// g_pos[b, :, j] = -sum over anchors m in increasing order, and picks near, far, out, of (a_m - p_j) * s_k where
+// pick_k(m) == j: positive-major, so every element is one fixed-order sum (no atomics, bit-reproducible).
+// Warp per positive keypoint; lane l keeps channels l, l+32, ... in registers (D <= USIP_CGF_MAX_D).
+__global__ void __launch_bounds__(CGF_WARPS * 32)
+desc_cgf_bwd_pos_kernel(const float* __restrict__ anc_desc, const float* __restrict__ pos_desc,
+                        const float* __restrict__ sigma, const int32_t* __restrict__ sel, const float* __restrict__ aux,
+                        const float* __restrict__ cloud, const float* __restrict__ g, float sigma_max,
+                        float* __restrict__ g_pos, int M, int D) {
+  constexpr int R = USIP_CGF_MAX_D / 32;
+  const int b = blockIdx.y, lane = threadIdx.x & 31;
+  const int j = blockIdx.x * CGF_WARPS + (threadIdx.x >> 5);
+  if (j >= M) return;
+  const float* ad = anc_desc + (size_t)b * D * M;
+  const float* pd = pos_desc + (size_t)b * D * M;
+  float p[R], acc[R];
+#pragma unroll
+  for (int i = 0; i < R; ++i) {
+    const int c = lane + 32 * i;
+    p[i] = c < D ? pd[(size_t)c * M + j] : 0.f;
+    acc[i] = 0.f;
+  }
+  for (int m0 = 0; m0 < M; m0 += 32) {
+    const int m = m0 + lane;
+    int4 pk = make_int4(-1, -1, -1, 0);
+    if (m < M) pk = *reinterpret_cast<const int4*>(sel + 4 * ((size_t)b * M + m));
+    const int hit = (pk.x == j ? 1 : 0) | (pk.y == j ? 2 : 0) | (pk.z == j ? 4 : 0);
+    float s[3] = {0.f, 0.f, 0.f};
+    unsigned todo = __ballot_sync(0xffffffffu, hit != 0);
+    if (hit) cgf_pair_scales(cgf_coef(g, sigma, cloud, sel, aux, sigma_max, b, (size_t)b * M + m), pk.w,
+                             *reinterpret_cast<const float4*>(aux + 4 * ((size_t)b * M + m)), s);
+    while (todo) {                                       // matching anchors in increasing order
+      const int src = __ffs(todo) - 1;
+      todo &= todo - 1;
+      const int h = __shfl_sync(0xffffffffu, hit, src);
+      const float s0 = __shfl_sync(0xffffffffu, s[0], src), s1 = __shfl_sync(0xffffffffu, s[1], src);
+      const float s2 = __shfl_sync(0xffffffffu, s[2], src);
+      const int mm = m0 + src;
+#pragma unroll
+      for (int i = 0; i < R; ++i) {
+        const int c = lane + 32 * i;
+        if (c < D) {
+          const float e = ad[(size_t)c * M + mm] - p[i];
+          if (h & 1) acc[i] -= e * s0;
+          if (h & 2) acc[i] -= e * s1;
+          if (h & 4) acc[i] -= e * s2;
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < R; ++i) {
+    const int c = lane + 32 * i;
+    if (c < D) g_pos[(size_t)b * D * M + (size_t)c * M + j] = acc[i];
+  }
+}
+
 // PointOnSurfaceLoss (losses.py:146-183) after the nearest-point search: p = pc[:, arg], n = sn[0:3, arg],
 //   u = (kp - p) / (||kp - p|| + 1e-7),  loss = (n . u)^2     (B,M); the arg-min is not differentiated.
 // backward (g given): d = kp - p, r = ||d||, e = r + 1e-7, s = n . u:
@@ -463,4 +674,50 @@ extern "C" int usip_point_on_surface(const float* kp, const float* pc, const flo
   USIP_REQUIRE(kp && pc && sn && arg && (loss || (g && g_kp)) && S >= 3, "point_on_surface: bad args");
   point_on_surface_kernel<<<cdiv(B * M, 256), 256, 0, (cudaStream_t)stream>>>(kp, pc, sn, arg, g, loss, g_kp, B, M, N, S);
   return check_launch("point_on_surface_kernel");
+}
+
+static int cgf_check(const void* const* ptrs, int n, int B, int M, int D, const char* what) {
+  for (int i = 0; i < n; ++i)
+    if (!ptrs[i]) return fail(what);
+  if (B < 1 || M < 1) return fail(what);
+  if (M > USIP_CGF_MAX_M) return fail(what);
+  if (D < 4 || D % 4 != 0 || D > USIP_CGF_MAX_D) return fail(what);
+  return 0;
+}
+
+extern "C" int usip_desc_cgf_f32(const float* anc_kp, const float* pos_kp, const float* anc_desc, const float* pos_desc,
+                                 const float* sigma, const float* u_near, const float* u_out, const float* u_sel,
+                                 float radius, float gamma, float sigma_max, float* loss, float* active, int32_t* sel,
+                                 float* aux, float* cloud, int B, int M, int D, void* stream) {
+  const void* ptrs[] = {anc_kp, pos_kp, anc_desc, pos_desc, sigma, u_near, u_out, u_sel, loss, active, sel, aux, cloud};
+  if (cgf_check(ptrs, 13, B, M, D, "desc_cgf: bad args (null operand, B or M < 1, M above USIP_CGF_MAX_M, or D not a "
+                                   "multiple of 4 in [4, USIP_CGF_MAX_D])"))
+    return -1;
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(sel) | reinterpret_cast<uintptr_t>(aux)) & 15) == 0,
+               "desc_cgf: sel and aux must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  desc_cgf_select_kernel<<<dim3(cdiv(M, CGF_WARPS), B), CGF_WARPS * 32, 0, st>>>(anc_kp, pos_kp, anc_desc, pos_desc, u_near,
+                                                                                 u_out, u_sel, radius, gamma, sel, aux, M, D);
+  if (int e = check_launch("desc_cgf_select_kernel")) return e;
+  desc_cgf_reduce_kernel<<<B, 256, 0, st>>>(sigma, sel, aux, sigma_max, loss, active, cloud, M);
+  return check_launch("desc_cgf_reduce_kernel");
+}
+
+extern "C" int usip_desc_cgf_bwd(const float* anc_desc, const float* pos_desc, const float* sigma, const int32_t* sel,
+                                 const float* aux, const float* cloud, const float* g_loss, float sigma_max, float* g_anc,
+                                 float* g_pos, int B, int M, int D, void* stream) {
+  const void* ptrs[] = {anc_desc, pos_desc, sigma, sel, aux, cloud, g_loss, g_anc, g_pos};
+  if (cgf_check(ptrs, 9, B, M, D, "desc_cgf_bwd: bad args (null operand, B or M < 1, M above USIP_CGF_MAX_M, or D not "
+                                  "a multiple of 4 in [4, USIP_CGF_MAX_D])"))
+    return -1;
+  USIP_REQUIRE(((reinterpret_cast<uintptr_t>(sel) | reinterpret_cast<uintptr_t>(aux)) & 15) == 0,
+               "desc_cgf_bwd: sel and aux must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  dim3 grid(cdiv(M, CGF_WARPS), B);
+  desc_cgf_bwd_anchor_kernel<<<grid, CGF_WARPS * 32, 0, st>>>(anc_desc, pos_desc, sigma, sel, aux, cloud, g_loss, sigma_max,
+                                                               g_anc, M, D);
+  if (int e = check_launch("desc_cgf_bwd_anchor_kernel")) return e;
+  desc_cgf_bwd_pos_kernel<<<grid, CGF_WARPS * 32, 0, st>>>(anc_desc, pos_desc, sigma, sel, aux, cloud, g_loss, sigma_max,
+                                                            g_pos, M, D);
+  return check_launch("desc_cgf_bwd_pos_kernel");
 }

@@ -441,19 +441,26 @@ __global__ void group_select4_kernel(const float* __restrict__ gmax, const float
 // for any C), then warp 0 merges the slices in row order.  Every comparison is the layer epilogue's strict `v > best` /
 // `v < best` from -inf / +inf, and a later slice only replaces an earlier one when strictly better, so the result is
 // that of one in-order scan: deterministic, independent of the launch shape.
+// ARG: also the row r < ratio that scan keeps (the first row of the extreme value; row 0 when no row beats the start
+// value: all -inf / NaN), emitted as the row in the whole group, r * sub + a_in[q*ratio + r] when the inputs carry
+// row-in-sub-group args, r when they do not.
 constexpr int GMC_WARPS = 8;
+template <bool ARG>
 __global__ void __launch_bounds__(GMC_WARPS * 32)
 group_max_combine_kernel(const float* __restrict__ gmax, const float* __restrict__ gmin, float* __restrict__ omax,
-                         float* __restrict__ omin, int ratio, int C) {
+                         float* __restrict__ omin, const int32_t* __restrict__ amax_in, const int32_t* __restrict__ amin_in,
+                         int32_t* __restrict__ amax_out, int32_t* __restrict__ amin_out, int ratio, int sub, int C) {
   __shared__ float smax[GMC_WARPS][128], smin[GMC_WARPS][128];
+  __shared__ int rmax[ARG ? GMC_WARPS : 1][128], rmin[ARG ? GMC_WARPS : 1][128];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const size_t q = blockIdx.x;
   const int c0 = blockIdx.y * 128 + lane;
   const int per = (ratio + GMC_WARPS - 1) / GMC_WARPS;
   const int r0 = min(ratio, w * per), r1 = min(ratio, r0 + per);
   float mx[4], mn[4];
+  int ax[4], an[4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) { mx[j] = -INFINITY; mn[j] = INFINITY; }
+  for (int j = 0; j < 4; ++j) { mx[j] = -INFINITY; mn[j] = INFINITY; ax[j] = -1; an[j] = -1; }
 #pragma unroll 4
   for (int r = r0; r < r1; ++r) {                              // unrolled: several rows' loads in flight (ratio M)
     const size_t row = (q * ratio + r) * (size_t)C;
@@ -462,13 +469,16 @@ group_max_combine_kernel(const float* __restrict__ gmax, const float* __restrict
       const int c = c0 + 32 * j;
       if (c < C) {
         const float a = __ldg(gmax + row + c);
-        if (a > mx[j]) mx[j] = a;
-        if (gmin) { const float b = __ldg(gmin + row + c); if (b < mn[j]) mn[j] = b; }
+        if (a > mx[j]) { mx[j] = a; if (ARG) ax[j] = r; }
+        if (gmin) { const float b = __ldg(gmin + row + c); if (b < mn[j]) { mn[j] = b; if (ARG) an[j] = r; } }
       }
     }
   }
 #pragma unroll
-  for (int j = 0; j < 4; ++j) { smax[w][lane + 32 * j] = mx[j]; smin[w][lane + 32 * j] = mn[j]; }
+  for (int j = 0; j < 4; ++j) {
+    smax[w][lane + 32 * j] = mx[j]; smin[w][lane + 32 * j] = mn[j];
+    if (ARG) { rmax[w][lane + 32 * j] = ax[j]; rmin[w][lane + 32 * j] = an[j]; }
+  }
   __syncthreads();
   if (w != 0) return;
 #pragma unroll
@@ -476,13 +486,19 @@ group_max_combine_kernel(const float* __restrict__ gmax, const float* __restrict
     const int c = c0 + 32 * j;
     if (c >= C) continue;
     float a = smax[0][lane + 32 * j], b = smin[0][lane + 32 * j];
+    int ia = ARG ? rmax[0][lane + 32 * j] : 0, ib = ARG ? rmin[0][lane + 32 * j] : 0;
     for (int s = 1; s < GMC_WARPS; ++s) {
       const float x = smax[s][lane + 32 * j], y = smin[s][lane + 32 * j];
-      if (x > a) a = x;
-      if (y < b) b = y;
+      if (x > a) { a = x; if (ARG) ia = rmax[s][lane + 32 * j]; }
+      if (y < b) { b = y; if (ARG) ib = rmin[s][lane + 32 * j]; }
     }
     omax[q * C + c] = a;
     if (omin) omin[q * C + c] = b;
+    if (ARG) {
+      ia = max(ia, 0); ib = max(ib, 0);
+      amax_out[q * C + c] = amax_in ? ia * sub + __ldg(amax_in + (q * ratio + ia) * (size_t)C + c) : ia;
+      if (omin) amin_out[q * C + c] = amin_in ? ib * sub + __ldg(amin_in + (q * ratio + ib) * (size_t)C + c) : ib;
+    }
   }
 }
 
@@ -737,8 +753,27 @@ extern "C" int usip_group_max_combine(const float* gmax, const float* gmin, floa
   USIP_REQUIRE(ratio >= 1 && Q_out >= 1 && C >= 1, "group_max_combine: ratio, Q_out and C must be positive");
   USIP_REQUIRE(cdiv(C, 128) <= 65535, "group_max_combine: C too large");
   dim3 grid((unsigned)Q_out, (unsigned)cdiv(C, 128));
-  group_max_combine_kernel<<<grid, GMC_WARPS * 32, 0, (cudaStream_t)stream>>>(gmax, gmin, out_max, out_min, ratio, C);
+  group_max_combine_kernel<false><<<grid, GMC_WARPS * 32, 0, (cudaStream_t)stream>>>(gmax, gmin, out_max, out_min, nullptr,
+                                                                                     nullptr, nullptr, nullptr, ratio, 1, C);
   return check_launch("group_max_combine_kernel");
+}
+
+extern "C" int usip_group_max_combine_arg(const float* gmax, const float* gmin, const int32_t* amax, const int32_t* amin,
+                                          float* out_max, float* out_min, int32_t* out_amax, int32_t* out_amin, int ratio,
+                                          int sub, int Q_out, int C, void* stream) {
+  USIP_REQUIRE(gmax && out_max && out_amax, "group_max_combine_arg: bad args (gmax, out_max and out_amax are required)");
+  USIP_REQUIRE(!gmin == !out_min && !gmin == !out_amin,
+               "group_max_combine_arg: bad args (gmin, out_min and out_amin come together)");
+  USIP_REQUIRE(!amin || (amax && gmin), "group_max_combine_arg: bad args (amin needs amax and gmin)");
+  USIP_REQUIRE(!amax || !gmin || amin, "group_max_combine_arg: bad args (amax with gmin needs amin)");
+  USIP_REQUIRE(ratio >= 1 && Q_out >= 1 && C >= 1, "group_max_combine_arg: ratio, Q_out and C must be positive");
+  USIP_REQUIRE(!amax || sub >= 1, "group_max_combine_arg: sub must be positive with sub-group args");
+  USIP_REQUIRE(!amax || (int64_t)ratio * sub <= INT32_MAX, "group_max_combine_arg: ratio * sub overflows the row index");
+  USIP_REQUIRE(cdiv(C, 128) <= 65535, "group_max_combine_arg: C too large");
+  dim3 grid((unsigned)Q_out, (unsigned)cdiv(C, 128));
+  group_max_combine_kernel<true><<<grid, GMC_WARPS * 32, 0, (cudaStream_t)stream>>>(gmax, gmin, out_max, out_min, amax, amin,
+                                                                                    out_amax, out_amin, ratio, sub, C);
+  return check_launch("group_max_combine_kernel<arg>");
 }
 
 extern "C" int usip_head_finalize(const float* out4, int ld, const float* cluster_mean, float sigma_lower_bound,

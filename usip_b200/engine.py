@@ -611,6 +611,16 @@ def detector_backward(net, ctx, g_kp, g_sig):
     return bw.result(net)
 
 
+def _combine_sub_groups(grp, ratio, sub, keep):
+    """Reduce the sub-group max / min (and, with keep, their args) of a group-max layer to whole groups, in place."""
+    with _Prof("group_max_combine"):
+        if keep:
+                grp["gmax"], grp["gmin"], grp["amax"], grp["amin"] = ops.group_max_combine_arg(
+                grp["gmax"], ratio, grp["gmin"], grp["amax"], grp["amin"], sub)
+        else:
+            grp["gmax"], grp["gmin"] = ops.group_max_combine(grp["gmax"], ratio, grp["gmin"])
+
+
 def _group_net_forward(R, net, rows, Bp, M, K, keep, out=None):
     """The grouped PointNet shared by DescriptorLiteOld (networks.py:375-381) and the ablation detectors
     RPN_Detector_KNN / RPN_Detector_Ball (networks.py:567-572, 695-700):
@@ -619,12 +629,13 @@ def _group_net_forward(R, net, rows, Bp, M, K, keep, out=None):
     descriptor (the raw group max is returned) and BN+ReLU in the detectors (max_k relu(bn(.)) is written to `out`).
     The reference calls these convolutions WITHOUT epoch: their BN momentum never decays.
     Balls of more than 128 rows (K a multiple of 64) take the layer epilogue's group max over 64-row sub-groups and reduce
-    each run of K/64 of them with usip_group_max_combine; that path has no arg outputs, so it is forward-only."""
+    each run of K/64 of them with usip_group_max_combine -- with keep, usip_group_max_combine_arg, whose args are rows of
+    the whole ball, so the backward sees the same [Q, C] amax / amin as for a direct group max."""
     dev = rows.device
     G, Q = Bp * M * K, Bp * M
     sub = K if K <= 128 else 64
-    if sub != K and (K % sub != 0 or keep):
-        raise NotImplementedError("group of %d rows: groups above 128 must be a multiple of 64 and run forward only" % K)
+    if K % sub != 0:
+        raise NotImplementedError("group of %d rows: groups above 128 must be a multiple of 64" % K)
     c1, c2, c3, c4, c5 = net.conv1, net.conv2, net.conv3, net.conv4, net.conv5
     D = c3.conv.weight.shape[0]
     Y1, bn1, _ = R.run(rows, G, _w2d(c1.conv.weight), c1.conv.bias.detach(), c1.norm, c1.norm.momentum, name="grp.conv1")
@@ -632,8 +643,7 @@ def _group_net_forward(R, net, rows, Bp, M, K, keep, out=None):
     Y3, bn3, grp3 = R.run(Y2, G, _w2d(c3.conv.weight), c3.conv.bias.detach(), c3.norm, c3.norm.momentum, prev=bn2,
                           group=sub, want_group=True, want_arg=keep, name="grp.conv3")
     if sub != K:
-        with _Prof("group_max_combine"):
-            grp3["gmax"], grp3["gmin"] = ops.group_max_combine(grp3["gmax"], K // sub, grp3["gmin"])
+        _combine_sub_groups(grp3, K // sub, sub, keep)
     amax = torch.empty((Q, D), dtype=f32, device=dev)
     ops.group_select(grp3["gmax"], grp3["gmin"], bn3.scale, bn3.shift, amax, Q, D)          # y_first_max (networks.py:377)
     W4 = _w2d(c4.conv.weight)
@@ -646,8 +656,9 @@ def _group_net_forward(R, net, rows, Bp, M, K, keep, out=None):
                           c5.norm.momentum if last_bn else 0.1, prev=bn4, group=sub, want_group=True, want_arg=keep,
                           write_y=last_bn and keep, name="grp.conv5")
     if sub != K:
-        with _Prof("group_max_combine"):
-            grp5["gmax"], grp5["gmin"] = ops.group_max_combine(grp5["gmax"], K // sub, grp5["gmin"] if last_bn else None)
+        if not last_bn:                                    # a linear conv5 is pooled by its max only
+            grp5["gmin"] = grp5["amin"] = None
+        _combine_sub_groups(grp5, K // sub, sub, keep)
     result = grp5["gmax"]
     if last_bn:
         C5 = c5.conv.weight.shape[0]
@@ -754,24 +765,31 @@ def _descriptor_balls(opt, x, sn, keypoints, permute_idx):
     return feats, rows
 
 
-def descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=True):
-    """DescriptorLiteOldGlobal.forward (models/networks.py:433-479) on the fused plan, forward only.  The grouped PointNet
+def descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=True, keep=False):
+    """DescriptorLiteOldGlobal.forward (models/networks.py:433-479) on the fused plan.  The grouped PointNet
     is DescriptorLiteOld's; then PPFNet's global context:
         g = max over the M keypoints of each cloud of the raw conv5 max          (usip_group_max_combine, ratio M)
         fc1 on cat(desc, g) = desc W1[:, :D]^T + (g W1[:, D:]^T)[row / M] + b  -> BN + ReLU
         fc2 -> BN + ReLU, fc3 linear, L2 normalisation.
     The EquivariantLayers are called without epoch, like the convolutions: their BN momentum never decays.
-    Returns (descriptor (B,D,M), x_features (B,3+S,M,K))."""
+    Returns (descriptor (B,D,M), x_features (B,3+S,M,K), ctx) -- ctx holds what descriptor_global_backward needs (keep=True:
+    every pool's arg, the global max's keypoint included)."""
     opt = net.opt
     dev = x.device
+    if keep and not net.training:
+        raise NotImplementedError("gradients through eval-mode BatchNorm are not part of the hot path "
+                                  "(the reference only back-propagates in train mode, keypoint_descriptor.py:466)")
     Bp, M, K = x.shape[0], keypoints.shape[2], opt.ball_nsamples
     Q = Bp * M
     R = LayerRunner(net, net.training, use_tc, dev)
     feats, rows = _descriptor_balls(opt, x, sn, keypoints, permute_idx)
-    local, gctx = _group_net_forward(R, net, rows, Bp, M, K, False, out=None)        # [Q, D] raw max of conv5
+    local, gctx = _group_net_forward(R, net, rows, Bp, M, K, keep, out=None)         # [Q, D] raw max of conv5
     D = gctx["D"]
     with _Prof("global_max"):
-        glob, _ = ops.group_max_combine(local, M)                                     # [Bp, D]
+        if keep:
+            glob, _, glob_arg, _ = ops.group_max_combine_arg(local, M)                # [Bp, D], keypoint of each max
+        else:
+            glob, _ = ops.group_max_combine(local, M)
     f1, f2, f3 = net.fc1, net.fc2, net.fc3
     W1 = _w2d(f1.conv.weight)
     U, _, _ = R.run(glob, Bp, _cols(W1, D), None, relu_in=False, name="fc1_global")   # cat(desc, global): global is LAST
@@ -782,7 +800,11 @@ def descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=
     desc = torch.empty((Bp, OUT.shape[1], M), dtype=f32, device=dev)
     _lib.check(_lib.load().usip_l2norm_to_bcm(ops._p(OUT), OUT.stride(0), ops._p(desc), None, Bp, M, OUT.shape[1],
                                               ops._stream()), "usip_l2norm_to_bcm")
-    return desc, feats
+    ctx = None
+    if keep:
+        ctx = dict(gctx)
+        ctx.update(use_tc=use_tc, local=local, glob=glob, glob_arg=glob_arg, Y1f=Y1, bn1f=bn1, Y2f=Y2, bn2f=bn2, OUT=OUT)
+    return desc, feats, ctx
 
 
 def _group_net_backward(bw, net, ctx, GY5):
@@ -820,4 +842,41 @@ def descriptor_backward(net, ctx, g_desc):
     check(lib.usip_groupmax_scatter_add(p(GY5), GY5.stride(0), p(G_y), p(grp5["amax"]), K, Q, D, s()), "usip_groupmax_scatter_add")
     _group_net_backward(bw, net, ctx, GY5)
     # conv1..conv4 biases sit in front of a train-mode BatchNorm: exactly zero gradient (left zero-initialised)
+    return bw.result(net)
+
+
+def descriptor_global_backward(net, ctx, g_desc):
+    """Backward of descriptor_global_forward (points / keypoints carry no gradient): gradients of net.parameters() in order.
+
+    desc = l2norm(fc3(a2)),  a2 = relu(bn2(fc2(a1))),  a1 = relu(bn1(local W1A^T + (g W1B^T)[row/M])),
+    g = max over the cloud's M keypoints of local,  local = max_k conv5(a4) (the grouped PointNet, networks.py:433-479)."""
+    dev = g_desc.device
+    Bp, M, K, D = ctx["Bp"], ctx["M"], ctx["K"], ctx["D"]
+    Q, G = Bp * M, Bp * M * K
+    bw = _Bwd(net, dev, ctx["use_tc"])
+    lib, check, p, s = bw.lib, bw.check, ops._p, ops._stream
+    f1, f2, f3 = net.fc1, net.fc2, net.fc3
+    OUT = ctx["OUT"]
+    # ---- L2 normalisation, fc3 (linear), fc2
+    G_out = torch.empty((Q, OUT.shape[1]), dtype=f32, device=dev)
+    check(lib.usip_l2norm_bwd(p(g_desc.contiguous()), p(OUT), OUT.stride(0), p(G_out), G_out.stride(0), Bp, M, OUT.shape[1],
+                              s()), "usip_l2norm_bwd")
+    GY = bw.conv_bwd(G_out, f3, Q, ctx["Y2f"], ctx["bn2f"], f2.norm, "fc3", "fc2")
+    GY = bw.conv_bwd(GY, f2, Q, ctx["Y1f"], ctx["bn1f"], f1.norm, "fc2", "fc1")
+    # ---- fc1 on cat(local, broadcast global max): the dense half, then the global half summed over each cloud's keypoints
+    local, glob = ctx["local"], ctx["glob"]
+    G_local = bw.conv_bwd(GY, f1, Q, local, cols=slice(0, D), name="fc1")                       # [Q, D]
+    G_U = torch.empty((Bp, GY.shape[1]), dtype=f32, device=dev)
+    check(lib.usip_group_sum(p(GY), GY.stride(0), p(G_U), G_U.stride(0), M, Bp, GY.shape[1], s()), "usip_group_sum")
+    GY.set_()                                   # frees GY's buffer even though the caller still holds the tensor
+    G_glob = bw.conv_bwd(G_U, f1, Bp, glob, cols=slice(D, None), name="fc1_global")             # [Bp, D]
+    # the global max is of the raw local descriptors: its gradient goes to each cloud's arg-max keypoint
+    check(lib.usip_groupmax_scatter_add(p(G_local), G_local.stride(0), p(G_glob), p(ctx["glob_arg"]), M, Bp, D, s()),
+          "usip_groupmax_scatter_add")
+    # ---- the max over each ball (conv5 is linear: the max of the raw output routes to its arg row)
+    GY5 = torch.zeros((G, D), dtype=f32, device=dev)
+    check(lib.usip_groupmax_scatter_add(p(GY5), GY5.stride(0), p(G_local), p(ctx["grp5"]["amax"]), K, Q, D, s()),
+          "usip_groupmax_scatter_add")
+    del G_local
+    _group_net_backward(bw, net, ctx, GY5)
     return bw.result(net)

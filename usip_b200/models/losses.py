@@ -3,9 +3,12 @@
   ChamferLoss_Brute            losses.py:44-99    probabilistic chamfer (sigma branch) + plain branch
   KeypointOnPCLoss             losses.py:102-116  (point_to_point -> SingleSideChamferLoss_Brute)
   SingleSideChamferLoss_Brute  losses.py:119-143
+  DescPairScanLoss             losses.py:190-237  outdoor descriptor triplet loss
+  DescCGFLoss                  losses.py:240-369  indoor descriptor triplet loss (CGF sampling)
 
 The (B,3,M,N) / (B,M,N) temporaries of the reference are never built: one tiled pairwise-L2 arg-min kernel
-(usip_pairwise_min_f32) serves all three, the reductions and the backward passes are small fused kernels.
+(usip_pairwise_min_f32) serves all three, the reductions and the backward passes are small fused kernels.  The descriptor
+losses likewise never build their (B,C,M,M) descriptor differences.
 """
 import ctypes
 
@@ -263,3 +266,66 @@ class DescPairScanLoss(nn.Module):
     def forward(self, anc_descriptors, pos_descriptors, neg_descriptors, anc_sigmas):
         return _DescTripletFn.apply(anc_descriptors, pos_descriptors, neg_descriptors, anc_sigmas.detach(),
                                     self.opt.triple_loss_gamma, self.opt.sigma_max)
+
+
+class _DescCGFFn(torch.autograd.Function):
+    """loss (B,M), active (B) of DescCGFLoss (usip_desc_cgf_f32); backward (usip_desc_cgf_bwd) to both descriptor sets
+    through the three selected pairs of every anchor."""
+
+    @staticmethod
+    def forward(ctx, module, anc_kp, anc_desc, pos_kp, pos_desc, sigmas, u_near, u_out, u_sel, radius, gamma, sigma_max):
+        a, p_ = anc_desc.contiguous(), pos_desc.contiguous()
+        sg = sigmas.contiguous()
+        from usip_b200 import engine
+        with engine._Prof("desc_cgf"):
+            loss, active, saved = ops.desc_cgf(anc_kp.contiguous(), pos_kp.contiguous(), a, p_, sg, (u_near, u_out, u_sel),
+                                               radius, gamma, sigma_max)
+        ctx.save_for_backward(a, p_, sg, *saved)
+        ctx.sigma_max = float(sigma_max)
+        module.last_picks = saved[0]
+        ctx.mark_non_differentiable(active)
+        return loss, active
+
+    @staticmethod
+    def backward(ctx, g_loss, g_active):
+        a, p_, sg, sel, aux, cloud = ctx.saved_tensors
+        from usip_b200 import engine
+        with engine._Prof("desc_cgf_bwd"):
+            g_a, g_p = ops.desc_cgf_bwd(a, p_, sg, (sel, aux, cloud), g_loss, ctx.sigma_max)
+        return None, None, g_a, None, g_p, None, None, None, None, None, None, None
+
+
+class DescCGFLoss(nn.Module):
+    """CGF triplet loss of the indoor descriptor (models/losses.py:240-369).  For every anchor keypoint (already mapped into
+    the positive frame): a random positive keypoint within CGF_radius, the closest one beyond it and a random one beyond
+    it; the negative is one of the latter two by a coin flip.  Loss (B,M) weighted by the anchor sigmas and rescaled by
+    the share of anchors that have a positive; active (B).  One kernel scans the (B,M,M) keypoint pairs without storing
+    them and computes only the three selected descriptor distances per anchor; the backward goes through those pairs.
+
+    The three random tensors are the reference's own torch.rand calls, same shapes, order and device (`draws`): with the
+    same CUDA seed the same GPU draws the same numbers.  `last_picks` holds the (B,M,4) int32 picks of the last call:
+    near, far, out and flags (bit 0: the anchor has a positive, bit 1: the negative is `far`)."""
+
+    def __init__(self, opt):
+        super().__init__()
+        self.opt = opt
+        self.last_picks = None
+
+    def draws(self, B, M, device):
+        """losses.py:279, 293, 298: u_near (B,M,M), u_out (B,M,M), u_sel (B,M), uniform in [0, 1)."""
+        u_near = torch.rand((B, M, M), dtype=torch.float32, device=device, requires_grad=False)
+        u_out = torch.rand((B, M, M), dtype=torch.float32, device=device, requires_grad=False)
+        u_sel = torch.rand((B, M), dtype=torch.float32, device=device, requires_grad=False)
+        return u_near, u_out, u_sel
+
+    def forward(self, anc_keypoints, anc_descriptors, pos_keypoints, pos_descriptors, anc_sigmas, anc_pc=None, pos_pc=None):
+        """anc_keypoints (B,3,M) in the positive frame, anc_descriptors (B,C,M), pos_keypoints (B,3,M), pos_descriptors
+        (B,C,M), anc_sigmas (B,M) -> (loss (B,M), active_percentage (B)).  anc_pc / pos_pc are accepted and unused, as in
+        the reference."""
+        B, _, M = anc_keypoints.shape
+        if not anc_descriptors.is_cuda:
+            raise NotImplementedError("the DescCGFLoss training step runs on CUDA tensors only; there is no CPU path")
+        u_near, u_out, u_sel = self.draws(B, M, anc_keypoints.device)
+        return _DescCGFFn.apply(self, anc_keypoints.detach(), anc_descriptors, pos_keypoints.detach(), pos_descriptors,
+                                anc_sigmas.detach().float(), u_near, u_out, u_sel, float(self.opt.CGF_radius),
+                                float(self.opt.triple_loss_gamma), float(self.opt.sigma_max))

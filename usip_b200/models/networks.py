@@ -5,7 +5,7 @@ in usip_b200/engine.py.
   RPN_Detector      models/networks.py:20-162   (C1=128, C2=512)
   RPN_DetectorLite  models/networks.py:165-307  (C1=64,  C2=256; same graph)
   DescriptorLiteOld models/networks.py:310-385
-  DescriptorLiteOldGlobal models/networks.py:388-479  (indoor: PPFNet global context; forward only)
+  DescriptorLiteOldGlobal models/networks.py:388-479  (indoor: PPFNet global context)
   RPN_Detector_KNN  models/networks.py:482-608  (ablation: 64 nearest points per node instead of the SOM assignment)
   RPN_Detector_Ball models/networks.py:611-738  (ablation: first 64 points within radius 2 of each node)
 """
@@ -254,12 +254,35 @@ class DescriptorLiteOld(_PackedWeightHooks, nn.Module):
         return desc, feats
 
 
+class _DescriptorGlobalFn(torch.autograd.Function):
+    """Whole-network autograd node of DescriptorLiteOldGlobal: forward = engine.descriptor_global_forward(keep=True),
+    backward = engine.descriptor_global_backward; gradients flow to the parameters only."""
+
+    @staticmethod
+    def forward(ctx, net, x, sn, keypoints, epoch, permute_idx, *params):
+        desc, feats, saved = engine.descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx,
+                                                              use_tc=net.use_tc, keep=True)
+        ctx.net = net
+        ctx.saved_plan = saved
+        ctx.mark_non_differentiable(feats)
+        return desc, feats
+
+    @staticmethod
+    def backward(ctx, g_desc, g_feats):
+        if ctx.saved_plan is None:
+            raise RuntimeError("descriptor forward ran without saving activations")
+        grads = engine.descriptor_global_backward(ctx.net, ctx.saved_plan, g_desc)
+        ctx.saved_plan = None
+        return (None, None, None, None, None, None) + tuple(grads)
+
+
 class DescriptorLiteOldGlobal(_PackedWeightHooks, nn.Module):
     """models/networks.py:388-479, the indoor descriptor: DescriptorLiteOld's grouped PointNet, then PPFNet's global
     context -- the max of the descriptors over the M keypoints of each cloud, concatenated to every keypoint's descriptor,
     fc1 (2D->2D), fc2 (2D->D), fc3 (D->D, linear) -- and L2 normalisation.  The global context is taken over the keypoints
     the forward is given.  forward(x, sn, keypoints, is_train, epoch) -> (descriptor (B,D,M), x_features (B,3+S,M,K)).
-    Forward only: training (DescCGFLoss and its backward) is not implemented."""
+    With gradients enabled and trainable parameters the forward keeps its activations and pool args, and autograd runs
+    engine.descriptor_global_backward (_DescriptorGlobalFn)."""
 
     def __init__(self, opt):
         super().__init__()
@@ -282,17 +305,25 @@ class DescriptorLiteOldGlobal(_PackedWeightHooks, nn.Module):
         if opt.activation != "relu" or opt.normalization != "batch":
             raise NotImplementedError("the H100 plan implements activation='relu', normalization='batch'")
         self.use_tc = bool(getattr(opt, "use_tensor_cores", True))
+        self._keep = False
         self._install_weight_hooks()
 
     def forward(self, x, sn, keypoints, is_train=False, epoch=None):
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("DescriptorLiteOldGlobal runs forward only: training the indoor descriptor "
-                                      "(DescCGFLoss and its backward) is a follow-up.  Call it under torch.no_grad() or "
-                                      "freeze its parameters")
+        params = tuple(self.parameters())
+        self._keep = torch.is_grad_enabled() and any(p.requires_grad for p in params)
         if not x.is_cuda:
+            if self._keep:
+                raise NotImplementedError("DescriptorLiteOldGlobal with gradients: the DescCGFLoss training step runs on "
+                                          "CUDA tensors only; there is no CPU path")
             raise RuntimeError("usip_b200 runs on CUDA tensors only (no CPU fallback)")
+        if self._keep and self.conv1.conv.weight.shape[0] < 32:
+            raise NotImplementedError("DescriptorLiteOldGlobal with gradients needs descriptor_len >= 128: the BatchNorm "
+                                      "backward kernels take layers of at least 32 channels (conv1 has descriptor_len/4)")
         N = x.size()[2]
         # host-side permutation, same RNG stream as the reference (networks.py:443)
         permute_idx = torch.from_numpy(np.random.permutation(N).astype(np.int64)).to(x.device)
         with torch.cuda.device(x.device):
-            return engine.descriptor_global_forward(self, x, sn, keypoints, epoch, permute_idx, use_tc=self.use_tc)
+            if self._keep:
+                return _DescriptorGlobalFn.apply(self, x, sn, keypoints, epoch, permute_idx, *params)
+            desc, feats, _ = engine.descriptor_global_forward(self, x, sn, keypoints, epoch, permute_idx, use_tc=self.use_tc)
+            return desc, feats

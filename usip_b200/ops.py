@@ -631,6 +631,35 @@ def group_max_combine(gmax, ratio, gmin=None):
     return omax, omin
 
 
+def group_max_combine_arg(gmax, ratio, gmin=None, amax=None, amin=None, sub=1):
+    """group_max_combine with arg outputs -> (omax, omin, oamax, oamin), oamax / oamin [Q, C] i32 the row of the result in
+    the whole group of ratio * sub rows: r * sub + amax[q*ratio + r] with the sub-groups' row-in-sub-group args amax /
+    amin, r without them (r: the first of the `ratio` input rows holding the max / min, 0 when none beats -inf / +inf)."""
+    _req(gmax, f32, "gmax")
+    for name, t, dt in (("gmin", gmin, f32), ("amax", amax, i32), ("amin", amin, i32)):
+        if t is not None:
+            _req(t, dt, name)
+            if t.shape != gmax.shape:
+                raise ValueError("%s %s must have gmax's shape %s" % (name, tuple(t.shape), tuple(gmax.shape)))
+    if amin is not None and (amax is None or gmin is None):
+        raise ValueError("group_max_combine_arg: amin needs amax and gmin")
+    if amax is not None and gmin is not None and amin is None:
+        raise ValueError("group_max_combine_arg: the sub-group args of gmin (amin) are missing")
+    R, C = gmax.shape
+    if ratio < 1 or R % ratio != 0:
+        raise ValueError("group_max_combine_arg: ratio %d must divide the %d rows" % (ratio, R))
+    Q = R // ratio
+    dev = gmax.device
+    omax = torch.empty((Q, C), dtype=f32, device=dev)
+    oamax = torch.empty((Q, C), dtype=i32, device=dev)
+    omin = None if gmin is None else torch.empty((Q, C), dtype=f32, device=dev)
+    oamin = None if gmin is None else torch.empty((Q, C), dtype=i32, device=dev)
+    check(_lib.load().usip_group_max_combine_arg(_p(gmax), _p(gmin), _p(amax), _p(amin), _p(omax), _p(omin), _p(oamax),
+                                                 _p(oamin), int(ratio), int(sub), Q, C, _stream()),
+          "usip_group_max_combine_arg")
+    return omax, omin, oamax, oamin
+
+
 def head_finalize(out4, cluster_mean, lb, B, M):
     kp = torch.empty((B, 3, M), dtype=f32, device=out4.device)
     sig = torch.empty((B, M), dtype=f32, device=out4.device)
@@ -687,3 +716,66 @@ def mean_scale(d, alpha):
     out = torch.empty((1,), dtype=f32, device=d.device)
     check(_lib.load().usip_mean_scale(_p(d), d.numel(), float(alpha), _p(out), _stream()), "usip_mean_scale")
     return out
+
+
+# DescCGFLoss kernels (include/usip_b200.h): the positive keypoints of a cloud are staged in shared memory, and the backward
+# keeps D/32 descriptor channels per lane in registers
+CGF_MAX_M = 2048
+CGF_MAX_D = 512
+
+
+def desc_cgf_check(anc_kp, pos_kp, anc_desc, pos_desc, sigma, draws):
+    """Host-side argument check of desc_cgf (no device needed): float32, contiguous, shapes (B,3,M), (B,D,M), (B,M) and
+    the draws (B,M,M), (B,M,M), (B,M); M <= CGF_MAX_M, D a multiple of 4 in [4, CGF_MAX_D].  -> (B, M, D)"""
+    B, _, M = anc_kp.shape
+    D = anc_desc.shape[1]
+    want = dict(anc_kp=(B, 3, M), pos_kp=(B, 3, M), anc_desc=(B, D, M), pos_desc=(B, D, M), sigma=(B, M),
+                u_near=(B, M, M), u_out=(B, M, M), u_sel=(B, M))
+    got = dict(anc_kp=anc_kp, pos_kp=pos_kp, anc_desc=anc_desc, pos_desc=pos_desc, sigma=sigma, u_near=draws[0],
+               u_out=draws[1], u_sel=draws[2])
+    for name, t in got.items():
+        if t.dtype != f32:
+            raise ValueError("desc_cgf: %s must be float32, got %s" % (name, t.dtype))
+        if not t.is_contiguous():
+            raise ValueError("desc_cgf: %s must be contiguous" % name)
+        if tuple(t.shape) != want[name]:
+            raise ValueError("desc_cgf: %s has shape %s, expected %s" % (name, tuple(t.shape), want[name]))
+    if B < 1 or M < 1:
+        raise ValueError("desc_cgf: empty batch (B=%d, M=%d)" % (B, M))
+    if M > CGF_MAX_M:
+        raise ValueError("desc_cgf: M=%d keypoints exceed the %d the kernel stages in shared memory" % (M, CGF_MAX_M))
+    if D % 4 != 0 or not 4 <= D <= CGF_MAX_D:
+        raise ValueError("desc_cgf: descriptor length D=%d must be a multiple of 4 in [4, %d]" % (D, CGF_MAX_D))
+    return B, M, D
+
+
+def desc_cgf(anc_kp, pos_kp, anc_desc, pos_desc, sigma, draws, radius, gamma, sigma_max):
+    """DescCGFLoss forward (usip_desc_cgf_f32) -> loss (B,M), active (B), saved = (sel (B,M,4) i32, aux (B,M,4) f32,
+    cloud (B,2) f32) for desc_cgf_bwd."""
+    B, M, D = desc_cgf_check(anc_kp, pos_kp, anc_desc, pos_desc, sigma, draws)
+    for name, t in (("anc_kp", anc_kp), ("anc_desc", anc_desc), ("u_near", draws[0])):
+        _req(t, f32, name)
+    dev = anc_kp.device
+    loss = torch.empty((B, M), dtype=f32, device=dev)
+    active = torch.empty((B,), dtype=f32, device=dev)
+    sel = torch.empty((B, M, 4), dtype=i32, device=dev)
+    aux = torch.empty((B, M, 4), dtype=f32, device=dev)
+    cloud = torch.empty((B, 2), dtype=f32, device=dev)
+    check(_lib.load().usip_desc_cgf_f32(_p(anc_kp), _p(pos_kp), _p(anc_desc), _p(pos_desc), _p(sigma), _p(draws[0]),
+                                        _p(draws[1]), _p(draws[2]), float(radius), float(gamma), float(sigma_max), _p(loss),
+                                        _p(active), _p(sel), _p(aux), _p(cloud), B, M, D, _stream()), "usip_desc_cgf_f32")
+    return loss, active, (sel, aux, cloud)
+
+
+def desc_cgf_bwd(anc_desc, pos_desc, sigma, saved, g_loss, sigma_max):
+    """DescCGFLoss backward (usip_desc_cgf_bwd) -> g_anc, g_pos (B,D,M)."""
+    sel, aux, cloud = saved
+    B, D, M = anc_desc.shape
+    g = g_loss.contiguous().float()
+    if tuple(g.shape) != (B, M):
+        raise ValueError("desc_cgf_bwd: g_loss has shape %s, expected %s" % (tuple(g.shape), (B, M)))
+    g_anc = torch.empty_like(anc_desc)
+    g_pos = torch.empty_like(pos_desc)
+    check(_lib.load().usip_desc_cgf_bwd(_p(anc_desc), _p(pos_desc), _p(sigma), _p(sel), _p(aux), _p(cloud), _p(g),
+                                        float(sigma_max), _p(g_anc), _p(g_pos), B, M, D, _stream()), "usip_desc_cgf_bwd")
+    return g_anc, g_pos
