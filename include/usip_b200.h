@@ -77,6 +77,12 @@ int usip_knn_group_f32(const float* xyz, const float* feat, const float* centers
  * np.minimum propagates a NaN distance, the kernel keeps the smaller value. */
 int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float* out_nodes, int B, int Ns, int k,
                  void* stream);
+/* usip_fps_f64: usip_fps_f32 on float64 points, pts (B, Ns, 3) f64 (data/scenenn_descriptor_loader.py samples the
+ * float64 ICP'd anchor): the same distance arithmetic, arg-max and minimum, so points that are float32 values give
+ * usip_fps_f32's indices.  out_nodes (B, 3, k) f32 casts of the selected points, or NULL.  Ns <= 8192; the points sit in
+ * 24 * Ns bytes of shared memory. */
+int usip_fps_f64(const double* pts, const int32_t* start, int32_t* out_idx, float* out_nodes, int B, int Ns, int k,
+                 void* stream);
 
 /* Training pairs on the device (csrc/pairgen.cu): the detector's data/kitti_detector_loader.py:101-259
  * (KittiLoader.__getitem__) and data/modelnet_shrec_loader.py:152-275 (ModelNet_Shrec_Loader.__getitem__), and the
@@ -142,10 +148,34 @@ int usip_fps_f32(const float* pts, const int32_t* start, int32_t* out_idx, float
  *   fl32(z * fl32(hs)), hs = params[b, 44].
  * usip_cloud_gather_candidates_zscaled: usip_cloud_gather_candidates with z multiplied by z_scale[c] (2*n_pairs) f32 in
  *   fp32, the height-scaled FPS input of the Oxford detector.
+ * usip_cloud_gather_candidates_icp_f64 (SceneNN descriptor, data/scenenn_descriptor_loader.py __getitem__): out_pts
+ *   (2*n_pairs, n_cand, 3) f64, usip_fps_f64's input.  Side 1 (the positive): the exact doubles of the fp32 rows.  Side 0
+ *   (the anchor): hom2cart(T @ [x y z 1]^T) with T = icp (n_pairs, 4, 4) f64 row-major of the pair, in this order: per
+ *   row r of T, h_r = fl(fma(z, T[r,2], fma(y, T[r,1], x * T[r,0])) + T[r,3]) (numpy's BLAS leaves the order open),
+ *   then h_0 / h_3, h_1 / h_3, h_2 / h_3, divided even when T's last row is [0 0 0 1].
+ * usip_scenenn_desc_pair_augment (SceneNNDescriptorLoader.__getitem__ with augment / augment_rot_only, then
+ *   transform_pc_pytorch on the positive): rows (2*n_pairs, N) as above, icp as above, cand_pts the gathered float64
+ *   candidates and node_idx (2*n_pairs, M) i32 the FPS selection into them (usip_fps_f64 out_idx), n_cand <= 8192 their
+ *   count; params (n_pairs, 48) f64 in usip_pair_augment's layout, the rotations, [27] scale and [28:31] shift shared by
+ *   the pair's two clouds, and [45] the pair's augmentation kind: 2 full (train split), 1 rotations only (val), any other
+ *   value none (test).  flags: the USIP_PAIR_ROT_* and USIP_PAIR_TRANSLATION bits; USIP_PAIR_TRAIN is ignored (the kind
+ *   decides).  sn = columns 3:3+S, 3 <= S <= 8.
+ *   - anchor pc: the ICP above in float64, then (kind >= 1) the rotations as data @ R and (kind 2) the scale and
+ *     (USIP_PAIR_TRANSLATION) the shift, all in float64, then one cast to fp32.  anchor sn[0:3]: the same ICP map
+ *     (translation included), rounded to fp32, then each rotation in float64 rounded to fp32.  Other sn columns as read.
+ *   - positive pc: in float64 from its first rotation on; without one, kind 2 scales it in fp32 (fl32(x * fl32(scale)))
+ *     and shifts it as fl32(x + shift).  positive sn as the anchor's, without the ICP.
+ *   - nodes: cand_pts[c, node_idx[c, i]], float64 through the rotations, scale and shift, then cast.
+ *   - no jitter term at all.  Then the positive's pc, sn[0:3] and nodes get the fp32 dst transform of usip_pair_augment.
+ *   -> anc/pos pc (n_pairs, 3, N), sn (n_pairs, S, N), node (n_pairs, 3, M), R (n_pairs, 3, 3), scale (n_pairs),
+ *      shift (n_pairs, 3, 1) f32: the eleven ModelDescriptorIndoor.set_input tensors without the keypoints and sigmas.
+ *   Refused (-1 before any launch): a null icp, S < 3 or S > 8, 3 + S > C, USIP_PAIR_ENU_TO_CAM or
+ *   USIP_PAIR_HEIGHT_SCALE, M > n_cand, n_pairs > 32767.
  * usip_scale_channel_f32: t (B, C, L) f32 in place, t[b, k, :] *= factor in fp32 (the descriptor batch's height
  *   scaling, oxford/train_descriptor.py).
  * Every cloud of the augment and gather calls is one grid row, so usip_pair_augment, usip_indoor_pair_augment,
- *   usip_desc_pair_augment, usip_modelnet_pair_augment and usip_cloud_gather_candidates(_zscaled) take n_pairs <= 32767 (-1 before any launch
+ *   usip_desc_pair_augment, usip_modelnet_pair_augment, usip_scenenn_desc_pair_augment and
+ *   usip_cloud_gather_candidates(_zscaled, _icp_f64) take n_pairs <= 32767 (-1 before any launch
  *   above it); usip_test_cloud_gather takes n_clouds <= 65535 and usip_scale_channel_f32 B <= 65535. */
 #define USIP_PAIR_TRAIN 1
 #define USIP_PAIR_ROT_HORIZONTAL 2
@@ -166,6 +196,15 @@ int usip_cloud_gather_candidates_zscaled(const float* scans, int C, const int64_
                                          const int32_t* scan_of_cloud, const int32_t* rows, const int32_t* cand,
                                          const float* z_scale, float* out_pts, int n_pairs, int N, int n_cand,
                                          void* stream);
+int usip_cloud_gather_candidates_icp_f64(const float* scans, int C, const int64_t* offsets,
+                                         const int32_t* scan_of_cloud, const int32_t* rows, const int32_t* cand,
+                                         const double* icp, double* out_pts, int n_pairs, int N, int n_cand,
+                                         void* stream);
+int usip_scenenn_desc_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
+                                   const int32_t* rows, const double* icp, const double* cand_pts,
+                                   const int32_t* node_idx, const double* params, int flags, int S, int n_pairs, int N,
+                                   int M, int n_cand, float* anc_pc, float* anc_sn, float* anc_node, float* pos_pc,
+                                   float* pos_sn, float* pos_node, float* R, float* scale, float* shift, void* stream);
 int usip_scale_channel_f32(float* t, int B, int C, int L, int k, float factor, void* stream);
 int usip_pair_augment(const float* scans, int C, const int64_t* offsets, const int32_t* scan_of_cloud,
                       const int32_t* rows, const float* nodes, const double* params, const double* jit_pc,

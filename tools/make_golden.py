@@ -648,6 +648,66 @@ def golden_indoor_pairs(ref):
     print("indoor_pairs.npz", os.path.getsize(os.path.join(OUT, "indoor_pairs.npz")) // 1024, "KB")
 
 
+# data/scenenn_descriptor_loader.py SceneNNDescriptorLoader.__getitem__ on a synthetic SceneNN tree
+# (usip_b200.data.scenenn_detector_loader.write_synthetic_scenenn with pairs): every positive frame the rigid image of its
+# anchor, icp_np the aligning transform.  Train frame 4 (and so its positive, frame 5) has fewer than SD_N rows.
+SD_N, SD_M, SD_SEED = 1024, 64, 8100
+SD_COUNTS = {"train": 8, "val": 4, "test": 14}
+SD_PAIRS = {"train": [(0, 1), (2, 3), (4, 5), (6, 7)], "val": [(0, 1), (2, 3)],
+            "test": [(2 * k, 2 * k + 1) for k in range(7)]}          # the test loader keeps pairs 0, 3, 6
+SD_CASES = {        # name: ([(split, item)], np seed, S, rot_horizontal, rot_3d, rot_perturbation, translation)
+    "train": ([("train", 0)], 81, 4, 1, 0, 1, 0),                     # scenenn/options_descriptor.py defaults
+    "rot3d": ([("train", 1)], 82, 4, 0, 1, 1, 1),
+    "s3": ([("train", 3)], 83, 3, 1, 0, 1, 0),
+    "short": ([("train", 2)], 84, 4, 1, 0, 1, 0),
+    "val": ([("val", 1)], 85, 4, 1, 0, 1, 0),
+    "test": ([("test", 1)], 86, 4, 1, 0, 1, 0),
+    "seq": ([("train", 0), ("val", 0)], 87, 4, 1, 0, 1, 1),
+    "wdiv": ([("train", 3)], 88, 4, 1, 0, 1, 0),                      # icp_np[3] replaced by SD_WDIV_ICP
+}
+SD_WDIV_ICP = np.array([[0.0, -1.0, 0.0, 0.5], [1.0, 0.0, 0.0, -0.25], [0.0, 0.0, 1.0, 0.125],
+                        [0.01, -0.02, 0.015, 1.1]])                    # last row not [0 0 0 1]: pins the w division
+
+
+def scenenn_desc_rows(split, i):
+    return 600 if (split, i) in (("train", 4), ("train", 5)) else 1300
+
+
+def golden_scenenn_descpairs(ref):
+    import importlib
+    import tempfile
+    from usip_b200.data.scenenn_detector_loader import write_synthetic_scenenn
+    sd = importlib.import_module("data.scenenn_descriptor_loader")
+    keys = ("anc_pc", "anc_sn", "anc_node", "pos_pc", "pos_sn", "pos_node", "R", "scale", "shift")
+    out = {"N": np.int64(SD_N), "M": np.int64(SD_M), "tree/seed": np.int64(SD_SEED),
+           "tree/counts": np.array([SD_COUNTS[k] for k in ("train", "val", "test")], dtype=np.int64),
+           "wdiv_icp": SD_WDIV_ICP}
+    for split, p in SD_PAIRS.items():
+        out["tree/pairs_" + split] = np.array(p, dtype=np.int64)
+    with tempfile.TemporaryDirectory() as root:
+        write_synthetic_scenenn(root, SD_COUNTS, scenenn_desc_rows, seed=SD_SEED, pairs=SD_PAIRS)
+        for name, (items, seed, S, rh, r3, rp, tp) in SD_CASES.items():
+            opt = ref_shim.make_opt(input_pc_num=SD_N, node_num=SD_M, surface_normal_len=S, rot_horizontal=bool(rh),
+                                    rot_3d=bool(r3), rot_perturbation=bool(rp), translation_perturbation=bool(tp))
+            loaders = {split: sd.SceneNNDescriptorLoader(root, split, opt) for split in SD_COUNTS}
+            if name == "wdiv":
+                loaders["train"].icp_np = loaders["train"].icp_np.copy()
+                loaders["train"].icp_np[3] = SD_WDIV_ICP
+            np.random.seed(seed)
+            res = [loaders[split][i] for split, i in items]
+            for k, vals in zip(keys, zip(*res)):
+                out[name + "/" + k] = np.stack([np.asarray(v.numpy() if torch.is_tensor(v) else v, dtype=np.float32)
+                                                for v in vals])
+            out[name + "/case"] = np.array([seed, S, rh, r3, rp, tp], dtype=np.int64)
+            out[name + "/split"] = np.array([split for split, _ in items])
+            out[name + "/item"] = np.array([i for _, i in items], dtype=np.int64)
+            out[name + "/frames"] = np.stack([loaders[split].pairs_np[i] for split, i in items]).astype(np.int64)
+            out[name + "/icp"] = np.stack([loaders[split].icp_np[i] for split, i in items]).astype(np.float64)
+            print("scenenn_descpairs", name, {k: out[name + "/" + k].shape for k in keys})
+    np.savez_compressed(os.path.join(OUT, "scenenn_descpairs.npz"), **out)
+    print("scenenn_descpairs.npz", os.path.getsize(os.path.join(OUT, "scenenn_descpairs.npz")) // 1024, "KB")
+
+
 # data/oxford_detector_loader.py OxfordLoader.__getitem__ and data/oxford_descriptor_loader.py OxfordDescriptorLoader
 # (items + default_collate + mine_negative_sample) on a synthetic Oxford tree (usip_b200.data.oxford_detector_loader.
 # write_synthetic_oxford): OX_TRAIN ENU scans along a line (positives within 2, non-negatives within 4), an invalid line

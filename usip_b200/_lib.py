@@ -60,6 +60,7 @@ SIGNATURES = {
     "usip_layer_tc_pack_many": (c_int, [ctypes.POINTER(LayerDesc), c_int, c_ptr]),
     "usip_layer_tile_rows": (c_int, []),
     "usip_fps_f32": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
+    "usip_fps_f64": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_pair_max_scan_rows": (c_int, []),
     "usip_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                   ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]
@@ -75,6 +76,10 @@ SIGNATURES = {
     "usip_cloud_gather_candidates": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_ptr]),
     "usip_cloud_gather_candidates_zscaled": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int,
                                                      c_int, c_ptr]),
+    "usip_cloud_gather_candidates_icp_f64": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int,
+                                                     c_int, c_ptr]),
+    "usip_scenenn_desc_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int,
+                                               c_int, c_int, c_int, c_int] + [c_ptr] * 9 + [c_ptr]),
     "usip_scale_channel_f32": (c_int, [c_ptr, c_int, c_int, c_int, c_int, ctypes.c_float, c_ptr]),
     "usip_desc_pair_augment": (c_int, [c_ptr, c_int, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                        ctypes.c_uint64, ctypes.c_uint64, c_int, c_int, c_int, c_int, c_int]

@@ -741,6 +741,147 @@ test_cloud_gather_kernel(const float* __restrict__ scans, int C, const int64_t* 
   }
 }
 
+// ------------------------------------------------------------------------ SceneNN descriptor pairs (ICP'd anchor)
+// data/scenenn_descriptor_loader.py's __getitem__ aligns the anchor to the positive with the pair's 4x4 ICP matrix T:
+// anc_pc = hom2cart(T @ [x y z 1]^T), float64 from here on, and anc_sn[:, 0:3] the same map, written back into the
+// float32 sn view.  np.dot goes through BLAS, whose summation order is unspecified; this is the order fixed here (the
+// order of a dgemm micro-kernel): per output row r, the fused multiply-add chain over k = 0, 1, 2, 3 started by a plain
+// product, the last term T[r, 3] * 1 (an FMA by 1 is one rounded add).  Then x/w, y/w, z/w with w the fourth row's
+// chain, divided literally (w is exactly 1 only when T's last row is [0 0 0 1]).
+__device__ __forceinline__ void pg_icp(const double* T, double x, double y, double z, double& X, double& Y, double& Z) {
+  double h[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    h[r] = __dadd_rn(__fma_rn(z, T[4 * r + 2], __fma_rn(y, T[4 * r + 1], __dmul_rn(x, T[4 * r]))), T[4 * r + 3]);
+  X = __ddiv_rn(h[0], h[3]); Y = __ddiv_rn(h[1], h[3]); Z = __ddiv_rn(h[2], h[3]);
+}
+
+// FPS input of the SceneNN descriptor: pts[c, j, :] = float64 xyz of rows[c, cand[c, j]], ICP'd on the anchor side
+// (c even, T = icp[c / 2]), the exact double of the fp32 row on the positive side.
+__global__ void pair_gather_icp_f64_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
+                                           const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
+                                           const int32_t* __restrict__ cand, const double* __restrict__ icp,
+                                           double* __restrict__ pts, int N, int n_cand) {
+  const int c = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_cand) return;
+  const int r = rows[(int64_t)c * N + cand[(int64_t)c * n_cand + j]];
+  const float* p = scans + (offsets[scan_of_cloud[c]] + r) * C;
+  double X = p[0], Y = p[1], Z = p[2];
+  if ((c & 1) == 0) pg_icp(icp + (int64_t)(c >> 1) * 16, p[0], p[1], p[2], X, Y, Z);
+  double* o = pts + ((int64_t)c * n_cand + j) * 3;
+  o[0] = X; o[1] = Y; o[2] = Z;
+}
+
+// SceneNNDescriptorLoader.augment / augment_rot_only of one float64 point (the ICP'd anchor's pc, every node): the
+// rotations (kind >= 1), then with the full augmentation (kind 2) the scale and, under USIP_PAIR_TRANSLATION, the
+// shift.  The loader draws its jitter but never adds it, so there is no jitter term (not even a zero: x + 0.0 would
+// turn -0.0 into +0.0).
+__device__ __forceinline__ void pg_scenenn_f64(int flags, int kind, const double* P, double& X, double& Y, double& Z) {
+  if (kind < 1) return;
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    if (flags & (USIP_PAIR_ROT_HORIZONTAL << r)) pg_rowvec(X, Y, Z, P + 9 * r);
+  if (kind < 2) return;
+  X = __dmul_rn(X, P[27]); Y = __dmul_rn(Y, P[27]); Z = __dmul_rn(Z, P[27]);
+  if (flags & USIP_PAIR_TRANSLATION) { X = __dadd_rn(X, P[28]); Y = __dadd_rn(Y, P[29]); Z = __dadd_rn(Z, P[30]); }
+}
+
+// sn columns 0:3 under the rotations (kind >= 1): a float32 view, rounded after every rotation; never scaled or shifted
+__device__ __forceinline__ void pg_scenenn_sn(int flags, int kind, const double* P, float* sn) {
+  if (kind < 1) return;
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    if (!(flags & (USIP_PAIR_ROT_HORIZONTAL << r))) continue;
+    double a = sn[0], bb = sn[1], cc = sn[2];
+    pg_rowvec(a, bb, cc, P + 9 * r);
+    sn[0] = (float)a; sn[1] = (float)bb; sn[2] = (float)cc;
+  }
+}
+
+// SceneNN descriptor pairs (scenenn_descriptor_loader.py:__getitem__, then transform_pc_pytorch on the positive).  The
+// pair's one set of rotations, scale and shift applies to both clouds; kind = params[b, 45] picks the augmentation:
+// 2 augment (train split), 1 augment_rot_only (val), anything else none (test).  The anchor's pc is float64 from its
+// ICP to the final cast; its sn[0:3] is ICP'd and rounded to fp32.  The positive's pc is the float32 slice until its
+// first rotation (then float64); un-rotated, the full augmentation scales it in fp32 and shifts it as fl32(x + shift).
+// Nodes are re-read as float64 FPS candidates (cand_pts[c, node_idx[c, i]]), so they stay float64 to the cast.
+__global__ void __launch_bounds__(PG_AUG_THREADS)
+scenenn_desc_pair_augment_kernel(const float* __restrict__ scans, int C, const int64_t* __restrict__ offsets,
+                                 const int32_t* __restrict__ scan_of_cloud, const int32_t* __restrict__ rows,
+                                 const double* __restrict__ icp, const double* __restrict__ cand_pts,
+                                 const int32_t* __restrict__ node_idx, const double* __restrict__ params, int flags,
+                                 int S, int N, int M, int n_cand, float* __restrict__ anc_pc, float* __restrict__ anc_sn,
+                                 float* __restrict__ anc_node, float* __restrict__ pos_pc, float* __restrict__ pos_sn,
+                                 float* __restrict__ pos_node, float* __restrict__ R_out, float* __restrict__ scale_out,
+                                 float* __restrict__ shift_out) {
+  const int c = blockIdx.y, b = c >> 1, side = c & 1;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const double* P = params + (int64_t)b * PG_PARAM_STRIDE;
+  const double* T = icp + (int64_t)b * 16;
+  const int kind = P[PG_AUGMENT_SLOT] == 2.0 ? 2 : (P[PG_AUGMENT_SLOT] == 1.0 ? 1 : 0);
+  float RT[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) RT[k] = (float)P[31 + k];
+
+  if (side == 1 && blockIdx.x == 0) {
+    if (threadIdx.x < 9) R_out[b * 9 + threadIdx.x] = RT[threadIdx.x];
+    else if (threadIdx.x == 9) scale_out[b] = (float)P[43];
+    else if (threadIdx.x < 13) shift_out[b * 3 + threadIdx.x - 10] = (float)P[40 + threadIdx.x - 10];
+  }
+
+  if (i < N) {
+    const float* p = scans + (offsets[scan_of_cloud[c]] + rows[(int64_t)c * N + i]) * C;
+    float x = p[0], y = p[1], z = p[2];
+    float sn[PG_MAX_S];
+#pragma unroll
+    for (int k = 0; k < PG_MAX_S; ++k) sn[k] = k < S ? p[3 + k] : 0.f;
+    if (side == 0) {                               // ICP'd, float64 to the cast
+      double X, Y, Z;
+      pg_icp(T, x, y, z, X, Y, Z);
+      pg_scenenn_f64(flags, kind, P, X, Y, Z);
+      x = (float)X; y = (float)Y; z = (float)Z;
+      double a, bb, cc;
+      pg_icp(T, sn[0], sn[1], sn[2], a, bb, cc);
+      sn[0] = (float)a; sn[1] = (float)bb; sn[2] = (float)cc;
+    } else if (kind >= 1 && (flags & PG_ANY_ROT)) {  // float64 after the first rotation
+      double X = x, Y = y, Z = z;
+      pg_scenenn_f64(flags, kind, P, X, Y, Z);
+      x = (float)X; y = (float)Y; z = (float)Z;
+    } else if (kind == 2) {                        // the float32 slice: fp32 scale, then fl32(x + shift)
+      const float scf = (float)P[27];
+      x = __fmul_rn(x, scf); y = __fmul_rn(y, scf); z = __fmul_rn(z, scf);
+      if (flags & USIP_PAIR_TRANSLATION) {
+        x = (float)__dadd_rn((double)x, P[28]); y = (float)__dadd_rn((double)y, P[29]);
+        z = (float)__dadd_rn((double)z, P[30]);
+      }
+    }
+    pg_scenenn_sn(flags, kind, P, sn);
+    float* opc = side ? pos_pc : anc_pc;
+    float* osn = side ? pos_sn : anc_sn;
+    if (side == 1) {                               // transform_pc_pytorch, fp32, column vectors
+      pg_dst_transform(RT, P, x, y, z);
+      pg_colvec(sn[0], sn[1], sn[2], RT);
+    }
+    opc[((int64_t)b * 3 + 0) * N + i] = x;
+    opc[((int64_t)b * 3 + 1) * N + i] = y;
+    opc[((int64_t)b * 3 + 2) * N + i] = z;
+#pragma unroll
+    for (int k = 0; k < PG_MAX_S; ++k)
+      if (k < S) osn[((int64_t)b * S + k) * N + i] = sn[k];
+  }
+
+  if (i < M) {
+    const double* q = cand_pts + ((int64_t)c * n_cand + node_idx[(int64_t)c * M + i]) * 3;
+    double X = q[0], Y = q[1], Z = q[2];
+    pg_scenenn_f64(flags, kind, P, X, Y, Z);
+    float x = (float)X, y = (float)Y, z = (float)Z;
+    if (side == 1) pg_dst_transform(RT, P, x, y, z);
+    float* ond = side ? pos_node : anc_node;
+    ond[((int64_t)b * 3 + 0) * M + i] = x;
+    ond[((int64_t)b * 3 + 1) * M + i] = y;
+    ond[((int64_t)b * 3 + 2) * M + i] = z;
+  }
+}
+
 // t[b, k, :] *= f in fp32 (torch's `t[:, k, :] *= f` with f a Python float: fl32(v * fl32(f)))
 __global__ void scale_channel_kernel(float* __restrict__ t, int C, int L, int k, float f) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -816,6 +957,45 @@ extern "C" int usip_cloud_gather_candidates_zscaled(const float* scans, int C, c
                                                     int n_pairs, int N, int n_cand, void* stream) {
   USIP_REQUIRE(z_scale, "cloud_gather_candidates_zscaled: null z_scale");
   return pg_gather(scans, C, offsets, scan_of_cloud, rows, cand, z_scale, out_pts, n_pairs, N, n_cand, stream);
+}
+
+extern "C" int usip_cloud_gather_candidates_icp_f64(const float* scans, int C, const int64_t* offsets,
+                                                    const int32_t* scan_of_cloud, const int32_t* rows,
+                                                    const int32_t* cand, const double* icp, double* out_pts,
+                                                    int n_pairs, int N, int n_cand, void* stream) {
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && cand && icp && out_pts,
+               "cloud_gather_candidates_icp_f64: null pointer");
+  USIP_REQUIRE(C >= 3 && n_pairs > 0 && N > 0 && n_cand > 0 && n_cand <= N,
+               "cloud_gather_candidates_icp_f64: bad sizes");
+  USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "cloud_gather_candidates_icp_f64: at most 32767 pairs");
+  dim3 grid(cdiv(n_cand, 256), 2 * n_pairs);
+  pair_gather_icp_f64_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(scans, C, offsets, scan_of_cloud, rows, cand, icp,
+                                                                      out_pts, N, n_cand);
+  return check_launch("pair_gather_icp_f64_kernel");
+}
+
+extern "C" int usip_scenenn_desc_pair_augment(const float* scans, int C, const int64_t* offsets,
+                                              const int32_t* scan_of_cloud, const int32_t* rows, const double* icp,
+                                              const double* cand_pts, const int32_t* node_idx, const double* params,
+                                              int flags, int S, int n_pairs, int N, int M, int n_cand, float* anc_pc,
+                                              float* anc_sn, float* anc_node, float* pos_pc, float* pos_sn,
+                                              float* pos_node, float* R, float* scale, float* shift, void* stream) {
+  USIP_REQUIRE(icp, "scenenn_desc_pair_augment: null icp");
+  USIP_REQUIRE(scans && offsets && scan_of_cloud && rows && cand_pts && node_idx && params,
+               "scenenn_desc_pair_augment: null input");
+  USIP_REQUIRE(anc_pc && anc_sn && anc_node && pos_pc && pos_sn && pos_node && R && scale && shift,
+               "scenenn_desc_pair_augment: null output");
+  USIP_REQUIRE(S >= 3 && S <= PG_MAX_S && 3 + S <= C,
+               "scenenn_desc_pair_augment: sn is columns 3:3+S (3 <= S <= 8, 3+S <= C)");
+  USIP_REQUIRE(!(flags & (USIP_PAIR_ENU_TO_CAM | USIP_PAIR_HEIGHT_SCALE)),
+               "scenenn_desc_pair_augment: the Oxford frame flags do not apply to indoor fragments");
+  USIP_REQUIRE(n_pairs > 0 && N > 0 && M > 0 && n_cand > 0 && M <= n_cand, "scenenn_desc_pair_augment: bad sizes");
+  USIP_REQUIRE(n_pairs <= PG_MAX_PAIRS, "scenenn_desc_pair_augment: at most 32767 pairs");
+  dim3 grid(cdiv(max(N, M), PG_AUG_THREADS), 2 * n_pairs);
+  scenenn_desc_pair_augment_kernel<<<grid, PG_AUG_THREADS, 0, (cudaStream_t)stream>>>(
+      scans, C, offsets, scan_of_cloud, rows, icp, cand_pts, node_idx, params, flags, S, N, M, n_cand, anc_pc, anc_sn,
+      anc_node, pos_pc, pos_sn, pos_node, R, scale, shift);
+  return check_launch("scenenn_desc_pair_augment_kernel");
 }
 
 extern "C" int usip_scale_channel_f32(float* t, int B, int C, int L, int k, float factor, void* stream) {

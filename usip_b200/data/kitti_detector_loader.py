@@ -151,7 +151,7 @@ class _PairBuilder:
     (side 0 = src / anchor, 1 = dst / positive) a subsample of one scan: subsets, FPS candidates and nodes are built per
     cloud, whichever scans a pair's two clouds come from.  A subclass names the scan of every cloud (`_clouds`), draws
     one pair's scalars (`_draw`) and runs its augment kernel (`_augment`); it may reorder parity mode's draws of one
-    item (`_draw_item`) and scale the FPS candidates' z (`_z_scale`).
+    item (`_draw_item`), scale the FPS candidates' z (`_z_scale`) or replace the candidates-to-nodes step (`_nodes`).
 
     rng="device": per-point randomness (subsets, jitter, FPS start) is Philox keyed by (seed, step, cloud, point,
     purpose); per-pair scalars come from a numpy RandomState seeded by (seed, step).  Host work is O(B) and a given
@@ -214,6 +214,14 @@ class _PairBuilder:
     def _z_scale(self, params):
         """(2B,) f32 factors of the FPS candidates' z, from the host params (B or 2B blocks), or None (no scaling)."""
         return None
+
+    def _nodes(self, scans, offsets, scan_of_cloud, rows, cand, start, params_h, up):
+        """Candidates -> FPS nodes: (the gathered FPS candidates, the nodes `_augment` takes).  By default the fp32
+        candidates (z scaled by `_z_scale`) and the (2B, 3, M) f32 nodes of usip_fps_f32.  up: host array -> device."""
+        zs = self._z_scale(params_h)
+        pts = ops.cloud_gather_candidates(scans, offsets, scan_of_cloud, rows, cand, None if zs is None else up(zs))
+        _, nodes = ops.fps(pts, start, self.M, want_nodes=True)
+        return pts, nodes
 
     def _build(self, scans, offsets, step, *items):
         offsets = np.asarray(offsets, dtype=np.int64)
@@ -283,10 +291,7 @@ class _PairBuilder:
             params_h = np.stack([d[0] for d in drawn])
             params_h = params_h.reshape(-1, params_h.shape[-1])
             params = up(params_h)
-            zs = self._z_scale(params_h)
-            pts = ops.cloud_gather_candidates(scans, offsets_d, scan_of_cloud, rows, cand,
-                                              None if zs is None else up(zs))
-            _, nodes = ops.fps(pts, start, M, want_nodes=True)
+            pts, nodes = self._nodes(scans, offsets_d, scan_of_cloud, rows, cand, start, params_h, up)
             out = self._augment(scans, offsets_d, scan_of_cloud, rows, nodes, params, step, jit)
         self.last = {"rows": rows, "cand": cand, "start": start, "candidates": pts, "params": params}
         return out

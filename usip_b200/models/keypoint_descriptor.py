@@ -186,9 +186,24 @@ class ModelDescriptorIndoor():
         z = lambda: torch.tensor([0], dtype=torch.float32, requires_grad=False, device=dev)
         self.test_loss_average = z(); self.test_loss_triplet_average = z(); self.test_active_percentage_average = z()
 
+    _INPUT_FIELDS = ("anc_pc", "anc_sn", "anc_keypoints", "anc_sigmas", "pos_pc", "pos_sn", "pos_keypoints",
+                     "pos_sigmas", "anc_R_pos", "anc_scale_pos", "anc_shift_pos")
+
     def set_input(self, anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas,
                   anc_R_pos, anc_scale_pos, anc_shift_pos):
-        """keypoint_descriptor.py:369-389."""
+        """keypoint_descriptor.py:369-389.  If the same tensors were staged by prefetch_input(), the staged device copies
+        are adopted with a stream-side wait instead of eleven copies and a host synchronisation."""
+        args = (anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas, anc_R_pos,
+                anc_scale_pos, anc_shift_pos)
+        st = getattr(self, "_staged", None)
+        if st is not None and len(st[0]) == len(args) and all(a is b for a, b in zip(st[0], args)):
+            cur = torch.cuda.current_stream()
+            cur.wait_event(st[2])
+            for k, v in zip(self._INPUT_FIELDS, st[1]):
+                v.record_stream(cur)                                  # allocated on another stream, consumed here
+                setattr(self, k, v)
+            self._staged = None
+            return
         dev = self.opt.device
         self.anc_pc = anc_pc.float().to(dev); self.anc_sn = anc_sn.float().to(dev)
         self.anc_keypoints = anc_keypoints.float().to(dev); self.anc_sigmas = anc_sigmas.float().to(dev)
@@ -197,6 +212,24 @@ class ModelDescriptorIndoor():
         self.anc_R_pos = anc_R_pos.float().to(dev); self.anc_scale_pos = anc_scale_pos.float().to(dev)
         self.anc_shift_pos = anc_shift_pos.float().to(dev)
         torch.cuda.synchronize()
+
+    def prefetch_input(self, *args, after=None):
+        """Not in the reference: stage the NEXT batch (the eleven set_input tensors) with asynchronous host-to-device
+        copies on a dedicated stream, so that the transfer overlaps the running step; the following set_input() with the
+        same tensor objects adopts the staged copies.  `after`: a CUDA event the staging waits for (device tensors
+        produced on another stream, e.g. by SceneNNDescriptorPairSource)."""
+        if len(args) != len(self._INPUT_FIELDS):
+            raise TypeError("prefetch_input takes the eleven set_input tensors, got %d" % len(args))
+        dev = self.opt.device
+        if getattr(self, "_copy_stream", None) is None:
+            self._copy_stream = torch.cuda.Stream(device=dev)
+        if after is not None:
+            self._copy_stream.wait_event(after)
+        with torch.cuda.stream(self._copy_stream):
+            staged = [a.float().to(dev, non_blocking=True).detach() for a in args]
+            ev = torch.cuda.Event()
+            ev.record(self._copy_stream)
+        self._staged = (tuple(args), staged, ev)
 
     def forward(self, pc, sn, keypoints, is_train=False, epoch=None):
         with torch.cuda.device(pc.get_device()):

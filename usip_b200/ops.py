@@ -138,6 +138,17 @@ def fps(pts, start, k, want_nodes=True):
     return idx, nodes
 
 
+def fps_f64(pts, start, k, want_nodes=False):
+    """fps on float64 points: pts (B,Ns,3) f64, start (B,) i32 -> (idx (B,k) i32, nodes (B,3,k) f32 casts or None)."""
+    _req(pts, torch.float64, "pts"); _req(start, i32, "start")
+    B, Ns, _ = pts.shape
+    idx = torch.empty((B, int(k)), dtype=i32, device=pts.device)
+    nodes = torch.empty((B, 3, int(k)), dtype=f32, device=pts.device) if want_nodes else None
+    with torch.cuda.device(pts.device):
+        check(_lib.load().usip_fps_f64(_p(pts), _p(start), _p(idx), _p(nodes), B, Ns, int(k), _stream()), "usip_fps_f64")
+    return idx, nodes
+
+
 # ----------------------------------------------------------------------------- training pairs (csrc/pairgen.cu)
 PAIR_TRAIN, PAIR_ROT_HORIZONTAL, PAIR_ROT_3D, PAIR_ROT_PERTURBATION, PAIR_TRANSLATION = 1, 2, 4, 8, 16
 PAIR_ENU_TO_CAM, PAIR_HEIGHT_SCALE = 32, 64      # Oxford: camera frame first; detector height scale = params[:, 44]
@@ -145,6 +156,7 @@ PAIR_PARAM_STRIDE = 48                           # detector: doubles per pair
 PAIR_AUGMENT_SLOT = 45                           # indoor_pair_augment: params[:, 45] != 0 augments the pair
 SUBSAMPLE_MAX_ROWS = 1 << 24                     # cloud_subsample: the longest scan (USIP_SUBSAMPLE_MAX_ROWS)
 DESC_PARAM_STRIDE = 32                           # descriptor: doubles per cloud
+SCENENN_KIND_NONE, SCENENN_KIND_ROT, SCENENN_KIND_FULL = 0, 1, 2   # scenenn_desc_pair_augment: params[:, 45]
 
 
 def pair_max_scan_rows():
@@ -204,6 +216,45 @@ def cloud_gather_candidates(scans, offsets, scan_of_cloud, rows, cand, z_scale=N
                                                            _p(rows), _p(cand), _p(z_scale), _p(pts), B, N, n_cand,
                                                            _stream()), "usip_cloud_gather_candidates_zscaled")
     return pts
+
+
+def _req_icp(icp, B):
+    _req(icp, torch.float64, "icp")
+    if tuple(icp.shape) != (B, 4, 4):
+        raise ValueError("icp must be (%d, 4, 4), one matrix per pair; got %s" % (B, tuple(icp.shape)))
+
+
+def cloud_gather_candidates_icp_f64(scans, offsets, scan_of_cloud, rows, cand, icp):
+    """SceneNN descriptor FPS input: (2B, n_cand, 3) f64 xyz of rows[c, cand[c, j]]; the anchor's (c even) mapped by
+    hom2cart(icp[c // 2] @ [x y z 1]) in the summation order of include/usip_b200.h, the positive's exact."""
+    _req_scans(scans, offsets, scan_of_cloud); _req(rows, i32, "rows"); _req(cand, i32, "cand")
+    B, N, n_cand = scan_of_cloud.shape[0] // 2, rows.shape[1], cand.shape[1]
+    _req_icp(icp, B)
+    pts = torch.empty((2 * B, n_cand, 3), dtype=torch.float64, device=scans.device)
+    with torch.cuda.device(scans.device):
+        check(_lib.load().usip_cloud_gather_candidates_icp_f64(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows), _p(cand), _p(icp), _p(pts), B, N,
+            n_cand, _stream()), "usip_cloud_gather_candidates_icp_f64")
+    return pts
+
+
+def scenenn_desc_pair_augment(scans, offsets, scan_of_cloud, rows, icp, cand_pts, node_idx, params, S, flags):
+    """SceneNN descriptor pairs -> (anc_pc, anc_sn, anc_node, pos_pc, pos_sn, pos_node, R (B,3,3), scale (B,),
+    shift (B,3,1)), all f32.  icp (B,4,4) f64, cand_pts (2B, n_cand, 3) f64 (cloud_gather_candidates_icp_f64), node_idx
+    (2B, M) i32 (fps_f64), params (B, 48) f64 with the pair's augmentation kind in params[:, PAIR_AUGMENT_SLOT]
+    (SCENENN_KIND_*).  No jitter: the reference loader draws it but never applies it."""
+    _req_scans(scans, offsets, scan_of_cloud); _req(rows, i32, "rows"); _req(node_idx, i32, "node_idx")
+    _req(cand_pts, torch.float64, "cand_pts"); _req(params, torch.float64, "params")
+    B, N, M, dev = scan_of_cloud.shape[0] // 2, rows.shape[1], node_idx.shape[1], scans.device
+    _req_icp(icp, B)
+    e = lambda *s: torch.empty(s, dtype=f32, device=dev)
+    out = (e(B, 3, N), e(B, S, N), e(B, 3, M), e(B, 3, N), e(B, S, N), e(B, 3, M), e(B, 3, 3), e(B), e(B, 3, 1))
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_scenenn_desc_pair_augment(
+            _p(scans), scans.shape[1], _p(offsets), _p(scan_of_cloud), _p(rows), _p(icp), _p(cand_pts), _p(node_idx),
+            _p(params), int(flags), int(S), B, N, M, cand_pts.shape[1], *[_p(t) for t in out], _stream()),
+            "usip_scenenn_desc_pair_augment")
+    return out
 
 
 def scale_channel_(t, k, factor):
