@@ -17,71 +17,36 @@ from usip_b200 import ops
 from usip_b200.optim import FlatAdam
 
 from . import losses, networks
-from ._common import random_point_dropout
+from ._common import StagedInput, random_point_dropout
 
 
-class ModelDescriptor():
-    def __init__(self, opt):
+class _ModelDescriptorBase(StagedInput):
+    """What the outdoor and indoor descriptor models share (keypoint_descriptor.py:14-318 and 321-603 are the same model
+    around a different network, loss and batch): each subclass gives its network and criterion classes, its extra batch
+    fields and `_loss()`."""
+    _INPUT_FIELDS = ("anc_pc", "anc_sn", "anc_keypoints", "anc_sigmas", "pos_pc", "pos_sn", "pos_keypoints",
+                     "pos_sigmas")
+
+    def __init__(self, opt, network, criterion):
         self.opt = opt
         if opt.gpu_ids[0] < 0:
-            raise RuntimeError("usip_b200.ModelDescriptor needs a CUDA device: there is no CPU path")
-        self.descriptor = networks.DescriptorLiteOld(opt).to(opt.device)
-        self.triplet_criteria = losses.DescPairScanLoss(opt)
+            raise RuntimeError("usip_b200.%s needs a CUDA device: there is no CPU path" % type(self).__name__)
+        self.descriptor = network(opt).to(opt.device)
+        self.triplet_criteria = criterion(opt)
         self.old_lr_descriptor = self.opt.lr
-        self.optimizer_descriptor = FlatAdam(self.descriptor.parameters(), lr=self.old_lr_descriptor,
-                                             betas=(0.9, 0.999), weight_decay=0)        # keypoint_descriptor.py:32-35
+        self.optimizer_descriptor = self._make_optimizer()
         dev = opt.device
         B, N, M = opt.batch_size, opt.input_pc_num, opt.node_num
         self.anc_pc = torch.empty(B, 3, N, device=dev).uniform_(); self.anc_sn = torch.empty(B, 3, N, device=dev).uniform_()
         self.anc_keypoints = torch.empty(B, 3, M, device=dev); self.anc_sigmas = torch.empty(B, M, device=dev)
         self.pos_pc = torch.empty(B, 3, N, device=dev).uniform_(); self.pos_sn = torch.empty(B, 3, N, device=dev).uniform_()
         self.pos_keypoints = torch.empty(B, 3, M, device=dev); self.pos_sigmas = torch.empty(B, M, device=dev)
-        self.neg_idx = torch.zeros(B, dtype=torch.long, device=dev)
         z = lambda: torch.tensor([0], dtype=torch.float32, requires_grad=False, device=dev)
         self.test_loss_average = z(); self.test_loss_triplet_average = z(); self.test_active_percentage_average = z()
 
-    _INPUT_FIELDS = ("anc_pc", "anc_sn", "anc_keypoints", "anc_sigmas", "pos_pc", "pos_sn", "pos_keypoints",
-                     "pos_sigmas", "neg_idx")
-
-    def set_input(self, anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas, neg_idx):
-        """keypoint_descriptor.py:77-107.  If the same tensors were staged by prefetch_input(), the staged device copies
-        are adopted with a stream-side wait instead of nine copies and a host synchronisation."""
-        args = (anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas, neg_idx)
-        st = getattr(self, "_staged", None)
-        if st is not None and len(st[0]) == len(args) and all(a is b for a, b in zip(st[0], args)):
-            cur = torch.cuda.current_stream()
-            cur.wait_event(st[2])
-            for k, v in zip(self._INPUT_FIELDS, st[1]):
-                v.record_stream(cur)                                  # allocated on another stream, consumed here
-                setattr(self, k, v)
-            self._staged = None
-            return
-        dev = self.opt.device
-        self.anc_pc = anc_pc.float().to(dev); self.anc_sn = anc_sn.float().to(dev)
-        self.anc_keypoints = anc_keypoints.float().to(dev); self.anc_sigmas = anc_sigmas.float().to(dev)
-        self.pos_pc = pos_pc.float().to(dev); self.pos_sn = pos_sn.float().to(dev)
-        self.pos_keypoints = pos_keypoints.float().to(dev); self.pos_sigmas = pos_sigmas.float().to(dev)
-        self.neg_idx = neg_idx.long().to(dev)
-        torch.cuda.synchronize()
-
-    def prefetch_input(self, *args, after=None):
-        """Not in the reference: stage the NEXT batch (the nine set_input tensors) with asynchronous host-to-device
-        copies on a dedicated stream, so that the transfer overlaps the running step; the following set_input() with the
-        same tensor objects adopts the staged copies.  `after`: a CUDA event the staging waits for (device tensors
-        produced on another stream, e.g. by KittiDescriptorPairSource).  neg_idx stays int64."""
-        if len(args) != len(self._INPUT_FIELDS):
-            raise TypeError("prefetch_input takes the nine set_input tensors, got %d" % len(args))
-        dev = self.opt.device
-        if getattr(self, "_copy_stream", None) is None:
-            self._copy_stream = torch.cuda.Stream(device=dev)
-        if after is not None:
-            self._copy_stream.wait_event(after)
-        with torch.cuda.stream(self._copy_stream):
-            staged = [a.float().to(dev, non_blocking=True).detach() for a in args[:-1]]
-            staged.append(args[-1].long().to(dev, non_blocking=True).detach())
-            ev = torch.cuda.Event()
-            ev.record(self._copy_stream)
-        self._staged = (tuple(args), staged, ev)
+    def _make_optimizer(self):
+        return FlatAdam(self.descriptor.parameters(), lr=self.old_lr_descriptor, betas=(0.9, 0.999),
+                        weight_decay=0)                 # keypoint_descriptor.py:32-35, 340-343
 
     def forward(self, pc, sn, keypoints, is_train=False, epoch=None):
         with torch.cuda.device(pc.get_device()):
@@ -93,34 +58,29 @@ class ModelDescriptor():
                                                   torch.cat(keypoints_tuple, dim=0), is_train, epoch)
         return torch.split(descriptors, n, dim=0), torch.split(x_aug_ball, n, dim=0)
 
-    def _loss(self):
-        triplet_loss, active_percentage = self.triplet_criteria(self.anc_descriptors, self.pos_descriptors,
-                                                                self.anc_descriptors[self.neg_idx, :, :], self.anc_sigmas)
-        self.triplet_loss = torch.mean(triplet_loss)
-        self.active_percentage = torch.mean(active_percentage)
-        self.loss = self.triplet_loss
+    def _run_siamese(self, is_train, epoch):
+        (self.anc_descriptors, self.pos_descriptors), _ = self.forward_siamese(
+            (self.anc_pc, self.pos_pc), (self.anc_sn, self.pos_sn), (self.anc_keypoints, self.pos_keypoints),
+            is_train=is_train, epoch=epoch)
 
     def optimize(self, epoch=None):
-        """keypoint_descriptor.py:126-157: optional random point dropout (same RNG streams), train-mode forward of the
-        (anchor, positive) batch, triplet loss against the in-batch negatives, backward, Adam."""
+        """keypoint_descriptor.py:126-157, 451-497: optional random point dropout (same RNG streams), train-mode forward
+        of the (anchor, positive) batch, the loss, backward, Adam."""
         with torch.cuda.device(self.anc_pc.get_device()):
             self.anc_pc, self.anc_sn, self.pos_pc, self.pos_sn = random_point_dropout(
                 self.opt, self.anc_pc, self.anc_sn, self.pos_pc, self.pos_sn)
             self.descriptor.train()
-            (self.anc_descriptors, self.pos_descriptors), _ = self.forward_siamese(
-                (self.anc_pc, self.pos_pc), (self.anc_sn, self.pos_sn), (self.anc_keypoints, self.pos_keypoints),
-                is_train=True, epoch=epoch)
+            self._run_siamese(is_train=True, epoch=epoch)
             self.optimizer_descriptor.zero_grad()
             self._loss()
             self.loss.backward()
             self.optimizer_descriptor.step()
 
     def test_model(self):
+        """Eval-mode forward and the loss; no parameter or running statistic changes."""
         self.descriptor.eval()
         with torch.cuda.device(self.anc_pc.device), torch.no_grad():
-            (self.anc_descriptors, self.pos_descriptors), _ = self.forward_siamese(
-                (self.anc_pc, self.pos_pc), (self.anc_sn, self.pos_sn), (self.anc_keypoints, self.pos_keypoints),
-                is_train=False, epoch=None)
+            self._run_siamese(is_train=False, epoch=None)
             self._loss()
 
     def freeze_model(self):
@@ -133,12 +93,8 @@ class ModelDescriptor():
             descriptors, _ = self.descriptor(pc, sn, keypoints, False, None)
         return descriptors
 
-    def get_negative_samples(self):
-        return (self.anc_pc[self.neg_idx, :, :], self.anc_sn[self.neg_idx, :, :],
-                self.anc_keypoints[self.neg_idx, :, :], self.anc_sigmas[self.neg_idx, :])
-
     def get_current_visuals(self):
-        raise NotImplementedError("visdom payloads (keypoint_descriptor.py:241-289) are outside the hot path")
+        raise NotImplementedError("visdom payloads (keypoint_descriptor.py:241-289, 540-572) are outside the hot path")
 
     def get_current_errors(self):
         return OrderedDict([('O_loss', self.loss.item()), ('O_triplet', self.triplet_loss.item()),
@@ -157,89 +113,54 @@ class ModelDescriptor():
         self.old_lr_descriptor = lr
 
 
-class ModelDescriptorIndoor():
+class ModelDescriptor(_ModelDescriptorBase):
+    """models/keypoint_descriptor.py:14-318: DescriptorLiteOld and DescPairScanLoss against in-batch negatives."""
+    _INPUT_FIELDS = _ModelDescriptorBase._INPUT_FIELDS + ("neg_idx",)
+    _INT64_FIELDS = ("neg_idx",)
+
+    def __init__(self, opt):
+        super().__init__(opt, networks.DescriptorLiteOld, losses.DescPairScanLoss)
+        self.neg_idx = torch.zeros(opt.batch_size, dtype=torch.long, device=opt.device)
+
+    def set_input(self, anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas, neg_idx):
+        """keypoint_descriptor.py:77-107."""
+        self._set_input((anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas, neg_idx))
+
+    def _loss(self):
+        triplet_loss, active_percentage = self.triplet_criteria(self.anc_descriptors, self.pos_descriptors,
+                                                                self.anc_descriptors[self.neg_idx, :, :], self.anc_sigmas)
+        self.triplet_loss = torch.mean(triplet_loss)
+        self.active_percentage = torch.mean(active_percentage)
+        self.loss = self.triplet_loss
+
+    def get_negative_samples(self):
+        return (self.anc_pc[self.neg_idx, :, :], self.anc_sn[self.neg_idx, :, :],
+                self.anc_keypoints[self.neg_idx, :, :], self.anc_sigmas[self.neg_idx, :])
+
+
+class ModelDescriptorIndoor(_ModelDescriptorBase):
     """models/keypoint_descriptor.py:321-603: DescriptorLiteOldGlobal and DescCGFLoss on the fused plan.  A module built on
     a CPU device constructs (for state_dict work) but has no optimizer and does not train."""
-
+    _INPUT_FIELDS = _ModelDescriptorBase._INPUT_FIELDS + ("anc_R_pos", "anc_scale_pos", "anc_shift_pos")
     _NO_CPU = "the DescCGFLoss training step runs on CUDA tensors only; there is no CPU path"
 
     def __init__(self, opt):
-        self.opt = opt
-        if opt.gpu_ids[0] < 0:
-            raise RuntimeError("usip_b200.ModelDescriptorIndoor needs a CUDA device: there is no CPU path")
-        self.descriptor = networks.DescriptorLiteOldGlobal(opt).to(opt.device)
-        self.triplet_criteria = losses.DescCGFLoss(opt)
-        self.old_lr_descriptor = self.opt.lr
-        dev = opt.device
-        self.optimizer_descriptor = None
-        if torch.device(dev).type == "cuda":                  # FlatAdam re-points CUDA parameters only
-            self.optimizer_descriptor = FlatAdam(self.descriptor.parameters(), lr=self.old_lr_descriptor,
-                                                 betas=(0.9, 0.999), weight_decay=0)    # keypoint_descriptor.py:340-343
-        B, N, M = opt.batch_size, opt.input_pc_num, opt.node_num
-        self.anc_pc = torch.empty(B, 3, N, device=dev).uniform_(); self.anc_sn = torch.empty(B, 3, N, device=dev).uniform_()
-        self.anc_keypoints = torch.empty(B, 3, M, device=dev); self.anc_sigmas = torch.empty(B, M, device=dev)
-        self.pos_pc = torch.empty(B, 3, N, device=dev).uniform_(); self.pos_sn = torch.empty(B, 3, N, device=dev).uniform_()
-        self.pos_keypoints = torch.empty(B, 3, M, device=dev); self.pos_sigmas = torch.empty(B, M, device=dev)
+        super().__init__(opt, networks.DescriptorLiteOldGlobal, losses.DescCGFLoss)
+        B, dev = opt.batch_size, opt.device
         self.anc_R_pos = torch.zeros((B, 3, 3), dtype=torch.float32, device=dev)
         self.anc_scale_pos = torch.zeros((B, 1), dtype=torch.float32, device=dev)
         self.anc_shift_pos = torch.zeros((B, 3, 1), dtype=torch.float32, device=dev)
-        z = lambda: torch.tensor([0], dtype=torch.float32, requires_grad=False, device=dev)
-        self.test_loss_average = z(); self.test_loss_triplet_average = z(); self.test_active_percentage_average = z()
 
-    _INPUT_FIELDS = ("anc_pc", "anc_sn", "anc_keypoints", "anc_sigmas", "pos_pc", "pos_sn", "pos_keypoints",
-                     "pos_sigmas", "anc_R_pos", "anc_scale_pos", "anc_shift_pos")
+    def _make_optimizer(self):
+        if torch.device(self.opt.device).type != "cuda":       # FlatAdam re-points CUDA parameters only
+            return None
+        return super()._make_optimizer()
 
     def set_input(self, anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas,
                   anc_R_pos, anc_scale_pos, anc_shift_pos):
-        """keypoint_descriptor.py:369-389.  If the same tensors were staged by prefetch_input(), the staged device copies
-        are adopted with a stream-side wait instead of eleven copies and a host synchronisation."""
-        args = (anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas, anc_R_pos,
-                anc_scale_pos, anc_shift_pos)
-        st = getattr(self, "_staged", None)
-        if st is not None and len(st[0]) == len(args) and all(a is b for a, b in zip(st[0], args)):
-            cur = torch.cuda.current_stream()
-            cur.wait_event(st[2])
-            for k, v in zip(self._INPUT_FIELDS, st[1]):
-                v.record_stream(cur)                                  # allocated on another stream, consumed here
-                setattr(self, k, v)
-            self._staged = None
-            return
-        dev = self.opt.device
-        self.anc_pc = anc_pc.float().to(dev); self.anc_sn = anc_sn.float().to(dev)
-        self.anc_keypoints = anc_keypoints.float().to(dev); self.anc_sigmas = anc_sigmas.float().to(dev)
-        self.pos_pc = pos_pc.float().to(dev); self.pos_sn = pos_sn.float().to(dev)
-        self.pos_keypoints = pos_keypoints.float().to(dev); self.pos_sigmas = pos_sigmas.float().to(dev)
-        self.anc_R_pos = anc_R_pos.float().to(dev); self.anc_scale_pos = anc_scale_pos.float().to(dev)
-        self.anc_shift_pos = anc_shift_pos.float().to(dev)
-        torch.cuda.synchronize()
-
-    def prefetch_input(self, *args, after=None):
-        """Not in the reference: stage the NEXT batch (the eleven set_input tensors) with asynchronous host-to-device
-        copies on a dedicated stream, so that the transfer overlaps the running step; the following set_input() with the
-        same tensor objects adopts the staged copies.  `after`: a CUDA event the staging waits for (device tensors
-        produced on another stream, e.g. by SceneNNDescriptorPairSource)."""
-        if len(args) != len(self._INPUT_FIELDS):
-            raise TypeError("prefetch_input takes the eleven set_input tensors, got %d" % len(args))
-        dev = self.opt.device
-        if getattr(self, "_copy_stream", None) is None:
-            self._copy_stream = torch.cuda.Stream(device=dev)
-        if after is not None:
-            self._copy_stream.wait_event(after)
-        with torch.cuda.stream(self._copy_stream):
-            staged = [a.float().to(dev, non_blocking=True).detach() for a in args]
-            ev = torch.cuda.Event()
-            ev.record(self._copy_stream)
-        self._staged = (tuple(args), staged, ev)
-
-    def forward(self, pc, sn, keypoints, is_train=False, epoch=None):
-        with torch.cuda.device(pc.get_device()):
-            return self.descriptor(pc, sn, keypoints, is_train, epoch)
-
-    def forward_siamese(self, pc_tuple, sn_tuple, keypoints_tuple, is_train=False, epoch=None):
-        n = pc_tuple[0].size()[0]
-        descriptors, x_aug_ball = self.descriptor(torch.cat(pc_tuple, dim=0), torch.cat(sn_tuple, dim=0),
-                                                  torch.cat(keypoints_tuple, dim=0), is_train, epoch)
-        return torch.split(descriptors, n, dim=0), torch.split(x_aug_ball, n, dim=0)
+        """keypoint_descriptor.py:369-389."""
+        self._set_input((anc_pc, anc_sn, anc_keypoints, anc_sigmas, pos_pc, pos_sn, pos_keypoints, pos_sigmas, anc_R_pos,
+                         anc_scale_pos, anc_shift_pos))
 
     def _require_cuda(self):
         if not self.anc_pc.is_cuda or self.optimizer_descriptor is None:
@@ -263,61 +184,14 @@ class ModelDescriptorIndoor():
         self.loss = self.triplet_loss
 
     def optimize(self, epoch=None):
-        """keypoint_descriptor.py:451-497: optional random point dropout (same RNG streams), train-mode forward of the
-        (anchor, positive) batch, DescCGFLoss, backward, Adam.  Nothing before the loss draws from the CUDA generator, so
-        the loss's three draws are the reference's."""
+        """Nothing before the loss draws from the CUDA generator, so the loss's three draws are the reference's."""
         self._require_cuda()
         if self.opt.random_pc_dropout_lower_limit < 0.99 and self.anc_pc.shape[2] != self.opt.input_pc_num:
             raise ValueError("ModelDescriptorIndoor.optimize: the staged batch has %d points, not input_pc_num=%d -- point "
                              "dropout thins the batch in place, so set_input() a new batch before every step"
                              % (self.anc_pc.shape[2], self.opt.input_pc_num))
-        with torch.cuda.device(self.anc_pc.get_device()):
-            self.anc_pc, self.anc_sn, self.pos_pc, self.pos_sn = random_point_dropout(
-                self.opt, self.anc_pc, self.anc_sn, self.pos_pc, self.pos_sn)
-            self.descriptor.train()
-            (self.anc_descriptors, self.pos_descriptors), _ = self.forward_siamese(
-                (self.anc_pc, self.pos_pc), (self.anc_sn, self.pos_sn), (self.anc_keypoints, self.pos_keypoints),
-                is_train=True, epoch=epoch)
-            self.optimizer_descriptor.zero_grad()
-            self._loss()
-            self.loss.backward()
-            self.optimizer_descriptor.step()
+        super().optimize(epoch)
 
     def test_model(self):
-        """keypoint_descriptor.py:499-519: eval-mode forward and the loss; no parameter or running statistic changes."""
         self._require_cuda()
-        self.descriptor.eval()
-        with torch.cuda.device(self.anc_pc.device), torch.no_grad():
-            (self.anc_descriptors, self.pos_descriptors), _ = self.forward_siamese(
-                (self.anc_pc, self.pos_pc), (self.anc_sn, self.pos_sn), (self.anc_keypoints, self.pos_keypoints),
-                is_train=False, epoch=None)
-            self._loss()
-
-    def freeze_model(self):
-        for p in self.descriptor.parameters():
-            p.requires_grad = False
-
-    def run_model(self, pc, sn, keypoints):
-        self.descriptor.eval()
-        with torch.cuda.device(pc.device), torch.no_grad():
-            descriptors, _ = self.descriptor(pc, sn, keypoints, False, None)
-        return descriptors
-
-    def get_current_visuals(self):
-        raise NotImplementedError("visdom payloads (keypoint_descriptor.py:540-572) are outside the hot path")
-
-    def get_current_errors(self):
-        return OrderedDict([('O_loss', self.loss.item()), ('O_triplet', self.triplet_loss.item()),
-                            ('O_active_perc', self.active_percentage.item()), ('E_loss', self.test_loss_average.item()),
-                            ('E_triplet', self.test_loss_triplet_average.item()),
-                            ('E_active_perc', self.test_active_percentage_average.item())])
-
-    def save_network(self, network, network_label, epoch_label, gpu_id):
-        torch.save(network.state_dict(), os.path.join(self.opt.checkpoints_dir, '%s_net_%s.pth' % (epoch_label, network_label)))
-
-    def update_learning_rate(self, ratio):
-        lr = max(self.old_lr_descriptor * ratio, 0.00001)
-        for g in self.optimizer_descriptor.param_groups:
-            g['lr'] = lr
-        print('update descriptor learning rate: %f -> %f' % (self.old_lr_descriptor, lr))
-        self.old_lr_descriptor = lr
+        super().test_model()

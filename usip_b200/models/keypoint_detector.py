@@ -17,10 +17,10 @@ from usip_b200 import _lib, engine, ops
 from usip_b200.optim import FlatAdam
 
 from . import losses, networks
-from ._common import random_point_dropout
+from ._common import StagedInput, random_point_dropout
 
 
-class ModelDetector():
+class ModelDetector(StagedInput):
     def __init__(self, opt):
         self.opt = opt
         if opt.scene == 'indoor':
@@ -75,7 +75,7 @@ class ModelDetector():
     def release_cuda_graphs(self):
         """Drop the captured step graphs (they are re-captured on demand).  A graph that holds an NCCL all-reduce must be
         destroyed BEFORE its communicator: call this (or usip_b200.dp.shutdown) ahead of destroy_process_group()."""
-        for k in ("_tgraph", "_tgraph_in", "_tgraph_out", "_graph", "_graph_in", "_graph_out"):
+        for k in ("_tgraph", "_graph"):
             self.__dict__.pop(k, None)
         if self._train_graph_key != "failed":
             self._train_graph_key = None
@@ -86,38 +86,8 @@ class ModelDetector():
     _INPUT_FIELDS = ("src_pc", "src_sn", "src_node", "dst_pc", "dst_sn", "dst_node", "src_R_dst", "src_scale_dst", "src_shift_dst")
 
     def set_input(self, src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, src_R_dst, src_scale_dst, src_shift_dst):
-        """keypoint_detector.py:120-134.  If the same host tensors were staged by prefetch_input(), the staged device
-        copies are adopted with a stream-side wait instead of nine copies and a host synchronisation."""
-        args = (src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, src_R_dst, src_scale_dst, src_shift_dst)
-        st = getattr(self, "_staged", None)
-        if st is not None and len(st[0]) == len(args) and all(a is b for a, b in zip(st[0], args)):
-            cur = torch.cuda.current_stream()
-            cur.wait_event(st[2])
-            for k, v in zip(self._INPUT_FIELDS, st[1]):
-                v.record_stream(cur)                                  # allocated on the copy stream, consumed here
-                setattr(self, k, v)
-            self._staged = None
-            return
-        dev = self.opt.device
-        for k, a in zip(self._INPUT_FIELDS, args):
-            setattr(self, k, a.float().to(dev, non_blocking=True).detach())
-        torch.cuda.synchronize()                                  # keypoint_detector.py:134
-
-    def prefetch_input(self, *args, after=None):
-        """Not in the reference: stage the NEXT batch (same nine tensors as set_input, ideally pinned) with asynchronous
-        host-to-device copies on a dedicated stream, so that the transfer overlaps the step that is running.  The
-        following set_input() with the same tensor objects adopts the staged copies.  `after`: a CUDA event the staging
-        waits for (device tensors produced on another stream, e.g. by DetectorPairBuilder)."""
-        dev = self.opt.device
-        if getattr(self, "_copy_stream", None) is None:
-            self._copy_stream = torch.cuda.Stream(device=dev)
-        if after is not None:
-            self._copy_stream.wait_event(after)
-        with torch.cuda.stream(self._copy_stream):
-            staged = [a.float().to(dev, non_blocking=True).detach() for a in args]
-            ev = torch.cuda.Event()
-            ev.record(self._copy_stream)
-        self._staged = (tuple(args), staged, ev)
+        """keypoint_detector.py:120-134."""
+        self._set_input((src_pc, src_sn, src_node, dst_pc, dst_sn, dst_node, src_R_dst, src_scale_dst, src_shift_dst))
 
     def forward(self, pc, sn, node, is_train=False, epoch=None):
         with torch.cuda.device(pc.get_device()):
@@ -268,62 +238,33 @@ class ModelDetector():
         engine.detector_backward(net, ctx, g_kp, g_sig)
 
     def _optimize_graph(self, epoch):
-        ins = [getattr(self, k) for k in self._GRAPH_INPUTS]
+        ins = [getattr(self, k) for k in self._INPUT_FIELDS]
         decays = any(getattr(m, "momentum_decay_step", None) for m in self.detector.modules())
         key = (tuple(tuple(t.shape) for t in ins), (None if epoch is None else int(epoch)) if decays else None,
                self._dp is not None, tuple(p.requires_grad for p in self.detector.parameters()))
         if self._train_graph_key != key:
+            opt_ = self.optimizer_detector
             try:
-                self._capture_train_step(key, ins, epoch)
+                # warm-up steps must not count as training: parameters, Adam state, the step counter and the BatchNorm
+                # buffers are restored afterwards
+                step = lambda: self._optimize_eager(epoch)
+                g = _StepGraph(self, step, [opt_.flat_p, opt_.exp_avg, opt_.exp_avg_sq, opt_.step_dev]
+                               + list(self.detector.buffers()))
+                _lib.WEIGHT_GEN[0] += 1                   # the capture must contain the weight (re-)packing kernels
+                g.capture(self, step)
             except Exception as e:                       # e.g. a collective that cannot be captured: keep training eagerly
                 import warnings
                 warnings.warn("usip_b200: CUDA-graph capture of the train step failed (%s: %s); running eagerly"
                               % (type(e).__name__, e))
                 self._train_graph_key = "failed"
                 torch.cuda.synchronize()
-                for k, v in zip(self._GRAPH_INPUTS, ins):
+                for k, v in zip(self._INPUT_FIELDS, ins):
                     setattr(self, k, v)
                 return self._optimize_eager(epoch)
+            self._tgraph, self._train_graph_key = g, key
         self.optimizer_detector.sync_hyperparams()        # lr lives in device memory; mirror it outside the graph
-        for dst, src in zip(self._tgraph_in, ins):
-            if dst.data_ptr() != src.data_ptr():
-                dst.copy_(src, non_blocking=True)
-        self._tgraph.replay()
-        _lib.LAUNCHES[0] += self._tgraph_launches
+        self._tgraph.replay(self, ins)
         _lib.WEIGHT_GEN[0] += 1                           # the replay moved the weights: packed tiles cached by eager paths are stale
-        for k, v in zip(self._GRAPH_INPUTS, self._tgraph_in):
-            setattr(self, k, v)
-        for k, v in self._tgraph_out.items():
-            setattr(self, k, v)
-
-    def _capture_train_step(self, key, ins, epoch):
-        opt_ = self.optimizer_detector
-        self._tgraph_in = [t.clone() for t in ins]
-        for k, v in zip(self._GRAPH_INPUTS, self._tgraph_in):
-            setattr(self, k, v)
-        # warm-up steps (allocator, kernel attributes) must not count as training: parameters, Adam state, the step
-        # counter and the BatchNorm buffers are restored afterwards
-        saved = [(t, t.detach().clone()) for t in [opt_.flat_p, opt_.exp_avg, opt_.exp_avg_sq, opt_.step_dev]
-                 + list(self.detector.buffers())]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self._optimize_eager(epoch)
-            with torch.no_grad():
-                for t, v in saved:
-                    t.copy_(v)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        _lib.WEIGHT_GEN[0] += 1                           # the capture must contain the weight (re-)packing kernels
-        g = torch.cuda.CUDAGraph()
-        n0 = _lib.LAUNCHES[0]
-        with torch.cuda.graph(g):
-            self._optimize_eager(epoch)
-        self._tgraph_launches = _lib.LAUNCHES[0] - n0
-        self._tgraph = g
-        self._tgraph_out = {k: getattr(self, k) for k in self._GRAPH_OUTPUTS}
-        self._train_graph_key = key
 
     def test_model(self):
         self.detector.eval()
@@ -331,8 +272,6 @@ class ModelDetector():
             self._run_siamese(is_train=False, epoch=None)
             self._losses()
 
-    _GRAPH_INPUTS = ("src_pc", "src_sn", "src_node", "dst_pc", "dst_sn", "dst_node",
-                     "src_R_dst", "src_scale_dst", "src_shift_dst")
     _GRAPH_OUTPUTS = ("src_node_recomputed", "dst_node_recomputed", "src_keypoints", "dst_keypoints", "src_sigmas",
                       "dst_sigmas", "src_keypoints_transformed", "loss_chamfer", "chamfer_pure", "chamfer_weighted",
                       "loss_keypoint_on_pc_src", "loss_keypoint_on_pc_dst", "loss")
@@ -353,49 +292,23 @@ class ModelDetector():
                 self._run_siamese(is_train=train_bn, epoch=epoch)
                 self._losses()
             return self.loss
-        ins = [getattr(self, k) for k in self._GRAPH_INPUTS]
+        ins = [getattr(self, k) for k in self._INPUT_FIELDS]
         key = (tuple(tuple(t.shape) for t in ins), bool(train_bn), epoch if epoch is None else int(epoch),
                tuple(p._version for p in self.detector.parameters()), _lib.WEIGHT_GEN[0])
         if getattr(self, "_graph_key", None) != key:
-            self._capture_forward_loss(key, ins, epoch, train_bn)
-        for dst, src in zip(self._graph_in, ins):
-            if dst.data_ptr() != src.data_ptr():
-                dst.copy_(src, non_blocking=True)
-        self._graph.replay()
-        _lib.LAUNCHES[0] += self._graph_launches
-        for k, v in zip(self._GRAPH_INPUTS, self._graph_in):
-            setattr(self, k, v)
-        for k, v in self._graph_out.items():
-            setattr(self, k, v)
+            def step():
+                with torch.no_grad():
+                    self._run_siamese(is_train=train_bn, epoch=epoch)
+                    self._losses()
+            # the warm-up passes must not count as training steps: BatchNorm running statistics (and
+            # num_batches_tracked) are restored afterwards, so a captured run leaves the same buffers behind as an eager one
+            g = _StepGraph(self, step, list(self.detector.buffers()))
+            g.capture(self, step)
+            self._graph = g
+            # the parameter versions may have been bumped by nothing here; recompute the key with the live versions
+            self._graph_key = key[:3] + (tuple(p._version for p in self.detector.parameters()), _lib.WEIGHT_GEN[0])
+        self._graph.replay(self, ins)
         return self.loss
-
-    def _capture_forward_loss(self, key, ins, epoch, train_bn):
-        self._graph_in = [t.clone() for t in ins]
-        for k, v in zip(self._GRAPH_INPUTS, self._graph_in):
-            setattr(self, k, v)
-        # the warm-up passes must not count as training steps: BatchNorm running statistics (and num_batches_tracked)
-        # are restored afterwards, so a captured run leaves the same buffers behind as an eager one
-        bn_buffers = [(b, b.detach().clone()) for b in self.detector.buffers()]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side), torch.no_grad():          # warm-up on a side stream (allocator, smem attributes,
-            for _ in range(2):                                   # packed-weight cache) before capture
-                self._run_siamese(is_train=train_bn, epoch=epoch)
-                self._losses()
-            for b, saved in bn_buffers:
-                b.copy_(saved)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        n0 = _lib.LAUNCHES[0]
-        with torch.cuda.graph(g), torch.no_grad():
-            self._run_siamese(is_train=train_bn, epoch=epoch)
-            self._losses()
-        self._graph_launches = _lib.LAUNCHES[0] - n0
-        self._graph = g
-        self._graph_out = {k: getattr(self, k) for k in self._GRAPH_OUTPUTS}
-        # the parameter versions may have been bumped by nothing here; recompute the key with the live versions
-        self._graph_key = (key[0], key[1], key[2], tuple(p._version for p in self.detector.parameters()), _lib.WEIGHT_GEN[0])
 
     def freeze_model(self):
         for p in self.detector.parameters():
@@ -443,3 +356,47 @@ class ModelDetector():
             param_group['lr'] = lr_detector
         print('update detector learning rate: %f -> %f' % (self.old_lr_detector, lr_detector))
         self.old_lr_detector = lr_detector
+
+
+class _StepGraph:
+    """One ModelDetector step captured as a CUDA graph over static copies of the step's inputs.  Construction binds the
+    copies to the model and runs the step twice on a side stream (allocator, kernel attributes, packed-weight cache); the
+    tensors in `restore` are then put back, so the warm-up leaves no trace.  `capture()` records the step; `replay()`
+    copies in the inputs that are not already the static ones, replays, and binds the static inputs and outputs to the
+    model.  The model is passed to each call rather than kept, so that the model and its graphs form no cycle."""
+
+    def __init__(self, model, step, restore):
+        self.ins = [getattr(model, k).clone() for k in model._INPUT_FIELDS]
+        for k, v in zip(model._INPUT_FIELDS, self.ins):
+            setattr(model, k, v)
+        saved = [(t, t.detach().clone()) for t in restore]
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                step()
+            with torch.no_grad():
+                for t, v in saved:
+                    t.copy_(v)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+
+    def capture(self, model, step):
+        g = torch.cuda.CUDAGraph()
+        n0 = _lib.LAUNCHES[0]
+        with torch.cuda.graph(g):
+            step()
+        self.launches = _lib.LAUNCHES[0] - n0
+        self.graph = g
+        self.outs = {k: getattr(model, k) for k in model._GRAPH_OUTPUTS}
+
+    def replay(self, model, ins):
+        for dst, src in zip(self.ins, ins):
+            if dst.data_ptr() != src.data_ptr():
+                dst.copy_(src, non_blocking=True)
+        self.graph.replay()
+        _lib.LAUNCHES[0] += self.launches
+        for k, v in zip(model._INPUT_FIELDS, self.ins):
+            setattr(model, k, v)
+        for k, v in self.outs.items():
+            setattr(model, k, v)
