@@ -368,6 +368,55 @@ int usip_fragment_overlap_f32(const float* xyz, const int64_t* offsets, int n_fr
 int usip_nms_f32(const float* keypoints, const float* sigmas, float radius, int32_t* out_idx, int32_t* out_count,
                  int B, int M, void* stream);
 
+/* Handcrafted keypoint baselines                              evaluation/save_keypoints.py:44-63, 289-331
+ * ('iss', 'harris', 'random' and ensure_keypoint_number).  Test clouds pc (B,3,N) f32, channel-major.
+ * Neighbour rule of every pass: j in N_r(i) <=> (dx*dx + dy*dy) + dz*dz in fp32 without FMA is <= fl32(r*r); i is in
+ * N_r(i); a row with a non-finite coordinate is in nobody's neighbourhood, gets count 0 and is never a keypoint.
+ * Every sum runs in an order fixed by the grid's cell contents, which usip_hc_grid_build fixes (entries of a cell in
+ * row order): results are bitwise repeatable, and rows with equal coordinates get bitwise-equal scores.
+ * Shapes: 1 <= B <= 65535, 1 <= N <= USIP_HC_MAX_POINTS, B*N <= USIP_HC_MAX_TOTAL; anything else is refused (-1).
+ * A radius must be finite and > 0.
+ *
+ * usip_hc_grid_build: the cell grid of every cloud (nngrid.cu's multi-CTA build, cells in row order) into `grid`,
+ *   usip_hc_grid_scratch_bytes(B, N) bytes (0 for a refused shape), 16-byte aligned.  The passes below read it; pass
+ *   them the same pc, B and N.
+ * usip_iss_saliency_f64 (PCL ISSKeypoint3D, no border estimation): C_i = sum over N_rs(i) of (p_j - p_i)(p_j - p_i)^T
+ *   in fp64 (unnormalised), eigenvalues e1 >= e2 >= e3 (fp64 Jacobi) -> saliency (B,N) f64 = e3 if |N_rs(i)| >=
+ *   min_neighbors, e2/e1 < gamma_21, e3/e2 < gamma_32 and e3 >= 0, else 0; count (B,N) i32 = |N_rs(i)| and eig (B,N,3)
+ *   f64 = (e1, e2, e3) are optional (NULL).  A non-finite row: saliency 0, count 0, eig 0.  Refused: gamma_21 or
+ *   gamma_32 outside (0, 1], min_neighbors < 1.
+ * usip_harris3d_response_f64 (PCL HarrisKeypoint3D, HARRIS response, no refinement): normals (B,N,3) f64 (written, the
+ *   caller's buffer) = unit eigenvector of the smallest eigenvalue of the mean-centred covariance of N_r(i), NaN when
+ *   |N_r(i)| < 3 (sign arbitrary); response (B,N) f64 = 0.04 + det(A) - 0.04 trace(A)^2 when trace(A) != 0, else 0,
+ *   A = mean of n_j n_j^T over j in N_r(i) with a finite n_j, NaN without one and for a non-finite row; count (B,N) i32
+ *   = |N_r(i)| (optional).
+ * usip_hc_nonmax (both detectors): flag (B,N) i32 = 1 where the row is finite, its score is eligible (score > threshold
+ *   when strict != 0, score >= threshold otherwise; NaN never), |N_r(i)| >= min_neighbors and no j in N_r(i) has
+ *   score_j > score_i (ties keep both, a NaN neighbour never suppresses); count (B,N) i32 = |N_r(i)| (optional).
+ *   ISS: score = saliency, radius = non_max_radius, threshold 0, strict, min_neighbors; Harris: score = response,
+ *   threshold, not strict, min_neighbors 1.  Refused: NaN threshold, min_neighbors < 1.
+ * usip_hc_select (ensure_keypoint_number for a whole keypoint-count sweep, one CTA per cloud): count (B,) i32 = the
+ *   flagged rows of each cloud (0 when flag is NULL: the 'random' method); order (B,L) i32 = first the min(count, L)
+ *   flagged rows in ascending (pg_random(seed, step, b, row, 7).x, row), then the L - min(count, L) smallest
+ *   (pg_random(seed, step, b, row, 8).x, row) over all N rows (pairgen.cu's counter layout, purposes 7 and 8).  A
+ *   K-prefix is K random keypoints, or every keypoint and K - count rows drawn without replacement from the cloud.
+ *   Refused: L < 1, L > N, L > USIP_HC_MAX_SELECT. */
+#define USIP_HC_MAX_POINTS (1 << 20)
+#define USIP_HC_MAX_TOTAL (1 << 26)
+#define USIP_HC_MAX_SELECT 4096
+size_t usip_hc_grid_scratch_bytes(int B, int N);
+int usip_hc_grid_build(const float* pc, void* grid, size_t grid_bytes, int B, int N, void* stream);
+int usip_iss_saliency_f64(const float* pc, const void* grid, size_t grid_bytes, int B, int N, float salient_radius,
+                          double gamma_21, double gamma_32, int min_neighbors, double* saliency, int32_t* count,
+                          double* eig, void* stream);
+int usip_harris3d_response_f64(const float* pc, const void* grid, size_t grid_bytes, int B, int N, float radius,
+                               double* normals, double* response, int32_t* count, void* stream);
+int usip_hc_nonmax(const float* pc, const void* grid, size_t grid_bytes, int B, int N, const double* score,
+                   float radius, double threshold, int strict, int min_neighbors, int32_t* flag, int32_t* count,
+                   void* stream);
+int usip_hc_select(const int32_t* flag, int B, int N, int L, uint64_t seed, uint64_t step, int32_t* order,
+                   int32_t* count, void* stream);
+
 /* operations.knn_gather_by_indexing                         models/operations.py:271-287
  * src (B,C,N), idx (B,M,K) i32 -> out (B,C,M,K): out[b,c,m,k] = src[b,c,idx[b,m,k]]. */
 int usip_knn_gather_f32(const float* src, const int32_t* idx, float* out,

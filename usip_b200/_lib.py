@@ -100,6 +100,15 @@ SIGNATURES = {
     "usip_fragment_overlap_f32": (c_int, [c_ptr, c_ptr, c_int, c_ptr, c_ptr, c_int, c_f32, c_ptr, ctypes.c_size_t, c_ptr,
                                           c_ptr]),
     "usip_nms_f32":(c_int, [c_ptr, c_ptr, ctypes.c_float, c_ptr, c_ptr, c_int, c_int, c_ptr]),
+    "usip_hc_grid_scratch_bytes": (ctypes.c_size_t, [c_int, c_int]),
+    "usip_hc_grid_build": (c_int, [c_ptr, c_ptr, ctypes.c_size_t, c_int, c_int, c_ptr]),
+    "usip_iss_saliency_f64": (c_int, [c_ptr, c_ptr, ctypes.c_size_t, c_int, c_int, c_f32, ctypes.c_double,
+                                      ctypes.c_double, c_int, c_ptr, c_ptr, c_ptr, c_ptr]),
+    "usip_harris3d_response_f64": (c_int, [c_ptr, c_ptr, ctypes.c_size_t, c_int, c_int, c_f32, c_ptr, c_ptr, c_ptr,
+                                           c_ptr]),
+    "usip_hc_nonmax": (c_int, [c_ptr, c_ptr, ctypes.c_size_t, c_int, c_int, c_ptr, c_f32, ctypes.c_double, c_int, c_int,
+                               c_ptr, c_ptr, c_ptr]),
+    "usip_hc_select": (c_int, [c_ptr, c_int, c_int, c_int, ctypes.c_uint64, ctypes.c_uint64, c_ptr, c_ptr, c_ptr]),
     "usip_l2norm_bwd": (c_int, [c_ptr, c_ptr, c_int, c_ptr, c_int, c_int, c_int, c_int, c_ptr]),
     "usip_desc_triplet_bwd": (c_int, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, ctypes.c_float, ctypes.c_float,
                                       c_ptr, c_ptr, c_ptr, c_ptr, c_int, c_int, c_int, c_int, c_int, c_ptr]),
@@ -185,7 +194,7 @@ def load():
 WEIGHT_GEN = [0]
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
-KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_cloud_subsample": 2, "usip_fragment_overlap_f32": 6, "usip_desc_cgf_f32": 2, "usip_desc_cgf_bwd": 2}
+KERNELS_PER_CALL = {"usip_cluster_sort": 3, "usip_pairwise_min_f32": 3, "usip_pairwise_min_grid_f32": 3, "usip_som_assign_grid_f32": 2, "usip_layer_fwd_tc": 2, "usip_ball_group_f32": 2, "usip_cloud_subsample": 2, "usip_fragment_overlap_f32": 6, "usip_desc_cgf_f32": 2, "usip_desc_cgf_bwd": 2, "usip_hc_grid_build": 3, "usip_harris3d_response_f64": 2}
 LAUNCHES = [0]
 
 

@@ -71,6 +71,17 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1
   return c;
 }
 
+// Counter layout of every per-point stream of pairgen.cu and handcrafted.cu: (item, cloud, step, purpose | sub << 8 |
+// step_hi << 16), key (seed_lo, seed_hi).  One purpose value per stream, so that no two streams share a counter.
+enum { PURPOSE_ROWS = 0, PURPOSE_CAND = 1, PURPOSE_START = 2, PURPOSE_JIT_PC = 3, PURPOSE_JIT_SN = 4,
+       PURPOSE_JIT_NODE = 5, PURPOSE_NOISE = 6, PURPOSE_HC_KEYPOINT = 7, PURPOSE_HC_PAD = 8 };
+
+__device__ __forceinline__ uint4 pg_random(uint64_t seed, uint64_t step, int cloud, int item, int purpose, int sub) {
+  const uint4 ctr = make_uint4((uint32_t)item, (uint32_t)cloud, (uint32_t)step,
+                               (uint32_t)purpose | ((uint32_t)sub << 8) | ((uint32_t)(step >> 32) << 16));
+  return philox4x32_10(ctr, (uint32_t)seed, (uint32_t)(seed >> 32));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

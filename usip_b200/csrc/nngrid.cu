@@ -12,36 +12,12 @@
 // Same arithmetic and tie rule as the brute-force kernels (csrc/loss.cu, csrc/group.cu): d2 = (dx*dx + dy*dy) + dz*dz without
 // FMA, smaller distance first, then smaller index; non-finite entries are never selected (their d2 is NaN or inf, which
 // `d < best` rejects in the reference formulation as well); a query with no selectable entry yields (inf, 0) / node 0.
-#include "common.cuh"
+#include "nngrid.cuh"
 
 namespace usip {
 
-constexpr int NG_MAXC = 8192;          // cells per cloud (two int arrays of this size live in shared memory while building)
-constexpr int NG_AXIS = 64;            // cells per axis at most
 constexpr int NG_BT = 1024;            // build threads
 constexpr int NG_MAXRING = 6;          // shells scanned before a query falls back to the whole (sorted) cloud
-
-struct NgGrid {
-  float ox, oy, oz, h, inv_h;
-  int nx, ny, nz;
-};
-
-static_assert(sizeof(NgGrid) == 32, "NgGrid is read as two 16-byte words");
-__device__ __forceinline__ NgGrid ng_load_grid(const NgGrid* p) {
-  const int4 a = __ldg(reinterpret_cast<const int4*>(p)), b = __ldg(reinterpret_cast<const int4*>(p) + 1);
-  NgGrid g;
-  g.ox = __int_as_float(a.x); g.oy = __int_as_float(a.y); g.oz = __int_as_float(a.z); g.h = __int_as_float(a.w);
-  g.inv_h = __int_as_float(b.x); g.nx = b.y; g.ny = b.z; g.nz = b.w;
-  return g;
-}
-
-__device__ __forceinline__ bool ng_finite3(float x, float y, float z) {
-  return (fabsf(x) <= 3.0e38f) && (fabsf(y) <= 3.0e38f) && (fabsf(z) <= 3.0e38f);    // false for NaN and inf
-}
-__device__ __forceinline__ int ng_cell1(float v, float o, float inv_h, int n) {
-  const float t = (v - o) * inv_h;
-  return (int)fminf(fmaxf(t, 0.f), (float)(n - 1));              // NaN -> 0 (callers filter non-finite values first)
-}
 
 // One CTA per cloud.  sorted[b][0..cnt) = (x, y, z, bits(n)) grouped by cell (x fastest), cell_start[b][0..ncell].
 __global__ void __launch_bounds__(NG_BT)
@@ -487,16 +463,49 @@ ng_assign_kernel(const float* __restrict__ xyz, int N, int M, const float4* __re
   if (count) atomicAdd(&count[(size_t)b * M + bi], 1);
 }
 
+// ---- the multi-CTA build as one call (usip_pairwise_min_grid_f32, handcrafted.cu)
+size_t ng_build_bytes(int B, int N) {
+  return (size_t)B * N * sizeof(float4) + 3 * (size_t)B * (NG_MAXC + 1) * sizeof(int32_t) + (size_t)B * sizeof(NgGrid) +
+         (size_t)B * N * sizeof(int32_t) + 128;
+}
+
+NgBuild ng_build_layout(void* scratch, int B, int N) {
+  NgBuild s;
+  s.sorted = reinterpret_cast<float4*>(scratch);
+  s.cell_start = reinterpret_cast<int32_t*>(s.sorted + (size_t)B * N);
+  NgGrid* grids = reinterpret_cast<NgGrid*>(s.cell_start + (size_t)B * (NG_MAXC + 1));
+  s.grids = reinterpret_cast<NgGrid*>((reinterpret_cast<uintptr_t>(grids) + 15) & ~(uintptr_t)15);
+  s.cnt = reinterpret_cast<int32_t*>(s.grids + B);
+  s.fill = s.cnt + (size_t)B * (NG_MAXC + 1);
+  s.cellid = s.fill + (size_t)B * (NG_MAXC + 1);
+  return s;
+}
+
+int ng_build_multi(const float* qry, int Ma, const float* pts, int N, int B, const NgBuild& s, cudaStream_t st) {
+  cudaError_t e = cudaMemsetAsync(s.cnt, 0, 2 * (size_t)B * (NG_MAXC + 1) * sizeof(int32_t), st);
+  if (e != cudaSuccess) { set_last_error("grid build: memset"); return (int)e; }
+  static bool attr = false;
+  const size_t smem = (size_t)(NG_MAXC + NG_MAXC / 32) * sizeof(int);
+  if (!attr) {
+    e = cudaFuncSetAttribute(ng_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_last_error("grid build: smem attribute"); return (int)e; }
+    attr = true;
+  }
+  const dim3 pgrid(cdiv(N, NGB_THREADS * NGB_PTS), B);
+  ng_bin_kernel<<<pgrid, NGB_THREADS, 0, st>>>(qry, Ma, pts, N, s.cellid, s.cnt, s.grids);
+  const dim3 sgrid(cdiv(N, NGB_THREADS * NGS_PTS), B);
+  ng_scatter_kernel<<<sgrid, NGB_THREADS, smem, st>>>(pts, N, s.cellid, s.cnt, s.fill, s.grids, s.cell_start, s.sorted);
+  return check_launch("grid build");
+}
+
 }  // namespace usip
 
 using namespace usip;
 
-// scratch layout: sorted float4 [B][N] | cell_start i32 [B][MAXC+1] | grids [B] | cnt i32 [B][MAXC+1] | fill i32 [B][MAXC+1] |
-// cellid i32 [B][N]
+// scratch layout: ng_build_layout (nngrid.cuh)
 extern "C" size_t usip_pairwise_min_grid_scratch_bytes(int B, int Nb) {
   if (B <= 0 || Nb <= 0) return 0;
-  return (size_t)B * Nb * sizeof(float4) + 3 * (size_t)B * (NG_MAXC + 1) * sizeof(int32_t) + (size_t)B * sizeof(NgGrid) +
-         (size_t)B * Nb * sizeof(int32_t) + 128;
+  return ng_build_bytes(B, Nb);
 }
 
 extern "C" int usip_pairwise_min_grid_f32(const float* a, const float* b, float* min_d, int32_t* arg, void* scratch,
@@ -505,28 +514,11 @@ extern "C" int usip_pairwise_min_grid_f32(const float* a, const float* b, float*
   USIP_REQUIRE(scratch_bytes >= usip_pairwise_min_grid_scratch_bytes(B, Nb), "pairwise_min_grid: scratch too small");
   USIP_REQUIRE((reinterpret_cast<uintptr_t>(scratch) & 15) == 0, "pairwise_min_grid: scratch must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  float4* sorted = reinterpret_cast<float4*>(scratch);
-  int32_t* cell_start = reinterpret_cast<int32_t*>(sorted + (size_t)B * Nb);
-  NgGrid* grids = reinterpret_cast<NgGrid*>(cell_start + (size_t)B * (NG_MAXC + 1));
-  grids = reinterpret_cast<NgGrid*>((reinterpret_cast<uintptr_t>(grids) + 15) & ~(uintptr_t)15);
-  int32_t* cnt = reinterpret_cast<int32_t*>(grids + B);
-  int32_t* fill = cnt + (size_t)B * (NG_MAXC + 1);
-  int32_t* cellid = fill + (size_t)B * (NG_MAXC + 1);
-  cudaError_t e = cudaMemsetAsync(cnt, 0, 2 * (size_t)B * (NG_MAXC + 1) * sizeof(int32_t), st);
-  if (e != cudaSuccess) { set_last_error("pairwise_min_grid: memset"); return (int)e; }
-  static bool attr = false;
-  const size_t smem = (size_t)(NG_MAXC + NG_MAXC / 32) * sizeof(int);
-  if (!attr) {
-    e = cudaFuncSetAttribute(ng_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { set_last_error("pairwise_min_grid: smem attribute"); return (int)e; }
-    attr = true;
-  }
-  const dim3 pgrid(cdiv(Nb, NGB_THREADS * NGB_PTS), B);
-  ng_bin_kernel<<<pgrid, NGB_THREADS, 0, st>>>(a, Ma, b, Nb, cellid, cnt, grids);
-  const dim3 sgrid(cdiv(Nb, NGB_THREADS * NGS_PTS), B);
-  ng_scatter_kernel<<<sgrid, NGB_THREADS, smem, st>>>(b, Nb, cellid, cnt, fill, grids, cell_start, sorted);
+  const NgBuild nb = ng_build_layout(scratch, B, Nb);
+  const int e = ng_build_multi(a, Ma, b, Nb, B, nb, st);
+  if (e != 0) return e;
   const int total = B * Ma;
-  ng_query_kernel<<<cdiv(total * 32, 256), 256, 0, st>>>(a, Ma, sorted, cell_start, grids, Nb, min_d, arg, total);
+  ng_query_kernel<<<cdiv(total * 32, 256), 256, 0, st>>>(a, Ma, nb.sorted, nb.cell_start, nb.grids, Nb, min_d, arg, total);
   return check_launch("pairwise_min_grid");
 }
 

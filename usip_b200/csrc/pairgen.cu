@@ -29,15 +29,7 @@ constexpr int PG_AUGMENT_SLOT = 45;                // usip_indoor_pair_augment: 
 constexpr int PG_DESC_PARAM_STRIDE = 32;           // doubles per cloud, see usip_desc_pair_augment in the header
 constexpr int PG_MAX_PAIRS = 32767;                // 2*n_pairs clouds run in grid.y, at most 65535
 
-enum { PURPOSE_ROWS = 0, PURPOSE_CAND = 1, PURPOSE_START = 2, PURPOSE_JIT_PC = 3, PURPOSE_JIT_SN = 4,
-       PURPOSE_JIT_NODE = 5, PURPOSE_NOISE = 6 };
-
-// ---------------------------------------------------------------------------------------------- Philox4x32-10
-__device__ __forceinline__ uint4 pg_random(uint64_t seed, uint64_t step, int cloud, int item, int purpose, int sub) {
-  const uint4 ctr = make_uint4((uint32_t)item, (uint32_t)cloud, (uint32_t)step,
-                               (uint32_t)purpose | ((uint32_t)sub << 8) | ((uint32_t)(step >> 32) << 16));
-  return philox4x32_10(ctr, (uint32_t)seed, (uint32_t)(seed >> 32));
-}
+// pg_random and the PURPOSE_* values live in common.cuh (handcrafted.cu draws from the same counter layout).
 
 // two standard normals from two 32-bit words (Box-Muller in double, u1 in (0, 1])
 __device__ __forceinline__ void pg_normal2(uint32_t a, uint32_t b, double& z0, double& z1) {

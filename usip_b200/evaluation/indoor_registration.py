@@ -47,6 +47,7 @@ import torch
 
 from usip_b200 import ops
 
+from .handcrafted import add_method_args, detector_from_args
 from .indoor_test_loader import MATCH3D_SCENES, REDWOOD_SCENES
 from .registration import Registration, _check_keypoint_limit, check_trials, descriptor_opt
 from .repeatability import (DEFAULT_KEYPOINT_NUMS, Match3DRepeatability, RedwoodRepeatability, check_sweep,
@@ -469,7 +470,7 @@ def main(argv=None):
     ap.add_argument("--root", help="redwood: numpy_gt_normal/; 3dmatch: 3DMatch_eval_npy/")
     ap.add_argument("--gt-root", help="redwood: the folder of original/<scene>-evaluation/{gt.log,gt.info}; 3dmatch: "
                                       "the folder of <scene>-evaluation/ (default --root)")
-    ap.add_argument("--detector", help="detector state dict (the reference's *_net_detector.pth)")
+    ap.add_argument("--detector", help="detector state dict (the reference's *_net_detector.pth); --method tsf only")
     ap.add_argument("--descriptor", help="descriptor state dict (the reference's *_net_descriptor.pth)")
     ap.add_argument("--descriptor-tree", metavar="DIR", help="score an existing result tree <DIR>/<scene>/<frame>.bin")
     ap.add_argument("--feature-dim", type=int, default=128, help="descriptor length of --descriptor-tree")
@@ -486,6 +487,7 @@ def main(argv=None):
     ap.add_argument("--input-pc-num", type=int, default=10240)
     ap.add_argument("--node-num", type=int, default=512)
     ap.add_argument("--json", metavar="OUT", help="write the summary as JSON")
+    add_method_args(ap)
     a = ap.parse_args(argv)
     if a.dataset == "redwood" and not a.gt_root:
         ap.error("redwood needs --gt-root")
@@ -506,8 +508,11 @@ def main(argv=None):
     check_trials(a.max_trials, INLIER_THRESHOLD)
     if not a.root:
         ap.error("give --root")
-    if not a.descriptor_tree and not (a.detector and a.descriptor):
-        ap.error("give --detector and --descriptor, or --descriptor-tree")
+    hc = detector_from_args(a, ap)
+    if not a.descriptor_tree and not ((a.detector or hc is not None) and a.descriptor):
+        ap.error("give --detector (--method tsf) and --descriptor, or --descriptor-tree")
+    if hc is not None and a.nms_radius >= 0.01:
+        ap.error("--nms-radius applies to --method tsf only")
     opt = descriptor_opt(a.dataset, batch_size=a.batch_size, input_pc_num=a.input_pc_num, node_num=a.node_num)
     kw = {"seed": a.seed, "batch_size": a.batch_size}
     if a.dataset == "redwood":
@@ -521,12 +526,16 @@ def main(argv=None):
         from usip_b200.models.keypoint_detector import ModelDetector
         from .registration import load_descriptor_checkpoint
         from .repeatability import load_detector_checkpoint
-        det, des = ModelDetector(opt), ModelDescriptorIndoor(opt)
-        load_detector_checkpoint(det, a.detector)
+        det = ModelDetector(opt) if hc is None else hc
+        des = ModelDescriptorIndoor(opt)
+        if hc is None:
+            load_detector_checkpoint(det, a.detector)
         load_descriptor_checkpoint(des, a.descriptor)
         ev.describe(det, des, a.nms_radius, L=ks[-1])
     res = ev.score(ks, a.max_trials, thr, a.pairs, a.seed)
     print("\n".join(res.lines()))
+    if hc is not None and not a.descriptor_tree:
+        print(hc.count_summary())
     if a.write_logs:
         ev.write_registration_logs(a.write_logs, ks[-1], a.max_trials[-1])
     if a.json:

@@ -42,6 +42,7 @@ import torch
 
 from usip_b200 import ops
 
+from .handcrafted import add_method_args, detector_from_args
 from .repeatability import (DEFAULT_KEYPOINT_NUMS, KittiRepeatability, OxfordRepeatability, check_sweep,
                             detector_opt, load_checkpoint, load_detector_checkpoint)
 
@@ -301,7 +302,7 @@ def main(argv=None):
                                  description="Registration of a trained detector and descriptor (evaluate_kitti.m / "
                                              "evaluate_oxford.m) on the KITTI or Oxford test set.")
     ap.add_argument("dataset", choices=("kitti", "oxford"))
-    ap.add_argument("--detector", help="detector state dict (the reference's *_net_detector.pth)")
+    ap.add_argument("--detector", help="detector state dict (the reference's *_net_detector.pth); --method tsf only")
     ap.add_argument("--descriptor", help="descriptor state dict (the reference's *_net_descriptor.pth)")
     ap.add_argument("--descriptor-tree", metavar="DIR", help="score an existing result tree instead")
     ap.add_argument("--feature-dim", type=int, default=128, help="descriptor length of --descriptor-tree")
@@ -323,11 +324,15 @@ def main(argv=None):
     ap.add_argument("--node-num", type=int, default=512)
     ap.add_argument("--write-descriptors", metavar="DIR", help="also write the result tree of the largest K")
     ap.add_argument("--json", metavar="OUT", help="write the summary as JSON")
+    add_method_args(ap)
     a = ap.parse_args(argv)
     _check_keypoint_limit(check_sweep(a.keypoint_nums, 1.0))
     check_trials(a.max_trials, a.inlier_threshold)
-    if not a.descriptor_tree and not (a.detector and a.descriptor):
-        ap.error("give --detector and --descriptor, or --descriptor-tree")
+    hc = detector_from_args(a, ap)
+    if not a.descriptor_tree and not ((a.detector or hc is not None) and a.descriptor):
+        ap.error("give --detector (--method tsf) and --descriptor, or --descriptor-tree")
+    if hc is not None and a.nms_radius >= 0.01:
+        ap.error("--nms-radius applies to --method tsf only")
     opt = descriptor_opt(a.dataset, batch_size=a.batch_size, input_pc_num=a.input_pc_num, node_num=a.node_num)
     if a.dataset == "kitti":
         if not (a.txt_root and a.numpy_root and a.calib_root):
@@ -344,12 +349,16 @@ def main(argv=None):
     else:
         from usip_b200.models.keypoint_descriptor import ModelDescriptor
         from usip_b200.models.keypoint_detector import ModelDetector
-        det, des = ModelDetector(opt), ModelDescriptor(opt)
-        load_detector_checkpoint(det, a.detector)
+        det = ModelDetector(opt) if hc is None else hc
+        des = ModelDescriptor(opt)
+        if hc is None:
+            load_detector_checkpoint(det, a.detector)
         load_descriptor_checkpoint(des, a.descriptor)
         res = ev.run(det, des, a.keypoint_nums, a.nms_radius, a.noise_sigma, a.max_trials, a.inlier_threshold,
                      a.match_k, a.seed)
     print("\n".join(res.lines()))
+    if hc is not None and not a.descriptor_tree:
+        print(hc.count_summary())
     if a.write_descriptors:
         ev.write_descriptor_tree(a.write_descriptors, a.keypoint_nums[-1])
     if a.json:

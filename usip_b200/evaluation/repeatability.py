@@ -41,6 +41,7 @@ import torch
 from usip_b200 import ops
 
 from .indoor_test_loader import MATCH3D_SCENES, REDWOOD_SCENES, Match3DTestLoader, RedwoodTestLoader
+from .handcrafted import add_method_args, detector_from_args
 from .kitti_test_loader import KittiTestLoader
 from .modelnet_test_loader import ModelNetRotatedTestLoader, eul2rotm, write_rotated_modelnet  # noqa: F401
 from .oxford_test_loader import OxfordTestLoader
@@ -228,6 +229,11 @@ class Repeatability:
         """Runs the detector over the whole test set and keeps every scan's keypoints (S, 3, M), sigmas (S, M) and
         selection order / count on the device.  With a ModelDescriptor `descriptor`, every batch is also described at
         its keypoints, on the clouds the detector saw (noise included), and descriptors (S, D, M) are kept too."""
+        if getattr(model, "handcrafted", False):
+            if nms_radius >= 0.01:
+                raise ValueError("nms_radius %g: the reference applies NMS to the learned detector only; a %s detector "
+                                 "runs with nms_radius < 0.01" % (nms_radius, model.method))
+            model.begin_pass()
         src = self.source
         dev = src.device
         S, M = len(src), src.M
@@ -419,7 +425,7 @@ def main(argv=None):
                                              "eval_rep.m) on the KITTI, Oxford, rotated ModelNet40, Redwood or 3DMatch "
                                              "test set.")
     ap.add_argument("dataset", choices=DATASETS)
-    ap.add_argument("--checkpoint", required=True, help="detector state dict (the reference's *_net_detector.pth)")
+    ap.add_argument("--checkpoint", help="detector state dict (the reference's *_net_detector.pth); --method tsf only")
     ap.add_argument("--txt-root", help="kitti: the folder of <seq>/groundtruths.txt and <seq>/correct_gt.txt")
     ap.add_argument("--numpy-root", help="kitti: the folder of <seq>/np_0.20_20480_r90_sn/%%06d.npy")
     ap.add_argument("--calib-root", help="kitti: the folder of <seq>/calib.txt")
@@ -440,9 +446,14 @@ def main(argv=None):
     ap.add_argument("--node-num", type=int, default=512)
     ap.add_argument("--write-keypoints", metavar="DIR", help="also write the .bin tree of the largest K")
     ap.add_argument("--json", metavar="OUT", help="write the summary as JSON")
+    add_method_args(ap)
     a = ap.parse_args(argv)
     check_sweep(a.keypoint_nums, a.inlier_radius)
-    from usip_b200.models.keypoint_detector import ModelDetector
+    hc = detector_from_args(a, ap)
+    if hc is None and not a.checkpoint:
+        ap.error("--method tsf needs --checkpoint")
+    if hc is not None and a.nms_radius >= 0.01:
+        ap.error("--nms-radius applies to --method tsf only")
     bs = a.batch_size or DEFAULT_BATCH_SIZE.get(a.dataset, 8)
     over = {"batch_size": bs, "node_num": a.node_num}
     if a.input_pc_num:
@@ -469,10 +480,16 @@ def main(argv=None):
         if not a.root:
             ap.error("3dmatch needs --root")
         ev = Match3DRepeatability(a.root, opt, gt_root=a.gt_root, **kw)
-    model = ModelDetector(opt)
-    load_detector_checkpoint(model, a.checkpoint)
+    if hc is None:
+        from usip_b200.models.keypoint_detector import ModelDetector
+        model = ModelDetector(opt)
+        load_detector_checkpoint(model, a.checkpoint)
+    else:
+        model = hc
     res = ev.run(model, a.keypoint_nums, a.nms_radius, a.inlier_radius, a.noise_sigma)
     print("\n".join(res.lines()))
+    if hc is not None:
+        print(hc.count_summary())
     if a.write_keypoints:
         ev.write_keypoint_tree(a.write_keypoints, a.keypoint_nums[-1])
     if a.json:

@@ -525,6 +525,87 @@ def nms(keypoints, sigmas, radius):
     return idx, cnt
 
 
+class HcGrid:
+    """The cell grid of a batch of test clouds (usip_hc_grid_build): pc (B,3,N) f32 CUDA and its scratch.  The radius
+    passes below take it so that one build serves every pass of a batch."""
+
+    def __init__(self, pc, scratch, nbytes):
+        self.pc, self.scratch, self.nbytes = pc, scratch, nbytes
+        self.B, self.N = pc.shape[0], pc.shape[2]
+
+
+def hc_grid(pc):
+    """usip_hc_grid_build: pc (B,3,N) f32 CUDA -> HcGrid."""
+    _req(pc, f32, "pc")
+    if pc.dim() != 3 or pc.shape[1] != 3:
+        raise ValueError("pc must be (B, 3, N)")
+    B, _, N = pc.shape
+    lib = _lib.load()
+    nbytes = int(lib.usip_hc_grid_scratch_bytes(B, N))
+    if nbytes == 0:
+        raise ValueError("hc_grid: B=%d, N=%d is outside the library's limits (include/usip_b200.h)" % (B, N))
+    scratch = torch.empty(((nbytes + 15) // 16, 4), dtype=i32, device=pc.device)
+    with torch.cuda.device(pc.device):
+        check(lib.usip_hc_grid_build(_p(pc), _p(scratch), nbytes, B, N, _stream()), "usip_hc_grid_build")
+    return HcGrid(pc, scratch, nbytes)
+
+
+def iss_saliency(grid, salient_radius, gamma_21, gamma_32, min_neighbors, want_eig=False):
+    """usip_iss_saliency_f64 -> (saliency (B,N) f64, count (B,N) i32 = |N_rs|, eig (B,N,3) f64 descending or None)."""
+    pc, B, N = grid.pc, grid.B, grid.N
+    sal = torch.empty((B, N), dtype=torch.float64, device=pc.device)
+    cnt = torch.empty((B, N), dtype=i32, device=pc.device)
+    eig = torch.empty((B, N, 3), dtype=torch.float64, device=pc.device) if want_eig else None
+    with torch.cuda.device(pc.device):
+        check(_lib.load().usip_iss_saliency_f64(_p(pc), _p(grid.scratch), grid.nbytes, B, N, float(salient_radius),
+                                                float(gamma_21), float(gamma_32), int(min_neighbors), _p(sal),
+                                                _p(cnt), _p(eig), _stream()), "usip_iss_saliency_f64")
+    return sal, cnt, eig
+
+
+def harris3d_response(grid, radius):
+    """usip_harris3d_response_f64 -> (response (B,N) f64, count (B,N) i32 = |N_r|, normals (B,N,3) f64)."""
+    pc, B, N = grid.pc, grid.B, grid.N
+    resp = torch.empty((B, N), dtype=torch.float64, device=pc.device)
+    cnt = torch.empty((B, N), dtype=i32, device=pc.device)
+    nrm = torch.empty((B, N, 3), dtype=torch.float64, device=pc.device)
+    with torch.cuda.device(pc.device):
+        check(_lib.load().usip_harris3d_response_f64(_p(pc), _p(grid.scratch), grid.nbytes, B, N, float(radius),
+                                                     _p(nrm), _p(resp), _p(cnt), _stream()),
+              "usip_harris3d_response_f64")
+    return resp, cnt, nrm
+
+
+def hc_nonmax(grid, score, radius, threshold, strict, min_neighbors):
+    """usip_hc_nonmax: score (B,N) f64 CUDA -> (flag (B,N) i32, count (B,N) i32 = |N_r|)."""
+    _req(score, torch.float64, "score")
+    pc, B, N = grid.pc, grid.B, grid.N
+    if tuple(score.shape) != (B, N):
+        raise ValueError("score must be (B, N)")
+    flag = torch.empty((B, N), dtype=i32, device=pc.device)
+    cnt = torch.empty((B, N), dtype=i32, device=pc.device)
+    with torch.cuda.device(pc.device):
+        check(_lib.load().usip_hc_nonmax(_p(pc), _p(grid.scratch), grid.nbytes, B, N, _p(score), float(radius),
+                                         float(threshold), 1 if strict else 0, int(min_neighbors), _p(flag), _p(cnt),
+                                         _stream()), "usip_hc_nonmax")
+    return flag, cnt
+
+
+def hc_select(flag, B, N, L, seed=0, step=0, device="cuda"):
+    """usip_hc_select: flag (B,N) i32 CUDA or None (random) -> (order (B,L) i32, count (B,) i32 flagged rows)."""
+    if flag is not None:
+        _req(flag, i32, "flag")
+        if tuple(flag.shape) != (B, N):
+            raise ValueError("flag must be (B, N)")
+        device = flag.device
+    order = torch.empty((B, int(L)), dtype=i32, device=device)
+    cnt = torch.empty((B,), dtype=i32, device=device)
+    with torch.cuda.device(order.device):
+        check(_lib.load().usip_hc_select(_p(flag), B, N, int(L), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1),
+                                         _p(order), _p(cnt), _stream()), "usip_hc_select")
+    return order, cnt
+
+
 def knn_gather(src, idx):
     _req(src, f32, "som_node"); _req(idx, i32, "som_node_knn_I")
     B, C, N = src.shape
