@@ -473,7 +473,9 @@ typedef struct usip_layer_desc {
   float* Y; int32_t ldy;               /* [P,Cout] output (NULL: not written)                         */
   float* stat_partial;                 /* [usip_layer_stat_slots(desc),2,Cout] partial (sum, sumsq) rows, or NULL */
   float* gmax; float* gmin;            /* [P/group,Cout] per-group max / min of Y, or NULL            */
-  int32_t* garg_max; int32_t* garg_min;/* [P/group,Cout] row-in-group of the max / min, or NULL       */
+  int32_t* garg_max; int32_t* garg_min;/* [P/group,Cout] row-in-group of the max / min, or NULL; on equal
+                                          values it is the FIRST such row of the group, on every kernel
+                                          (ball_pad repeats rows, so ties are real)                     */
   int32_t group;
   int32_t precision;                   /* 0 = fp32 SIMT, 1 = 3xTF32 wgmma (Cin%32==0, Cout%64==0) */
   void* tc_workspace;                  /* precision 1: >= usip_layer_tc_workspace_bytes(Cin,Cout) bytes */
@@ -704,7 +706,10 @@ int usip_head_bwd(const float* g_kp, const float* g_sig, const float* out4, int 
                   void* stream);
 /* gW[Cout,Cin] += GY[P,Cout]^T * act(X)[P,Cin], act = optional folded BN affine + ReLU (same prologue as forward);
  * precision 1: wgmma 3xTF32 (MN-major operands transposed to K-major in shared memory; precision 4: the same kernel as plain single-pass TF32) when Cout>=64, Cout%4==0, Cin%64==0, P>=4096 (a 64-wide layer fills half of the
- * 128-row tile (two m64 wgmma row blocks) with zero rows); Cin<=8 has an HBM-bound row-streaming kernel; otherwise the register-tiled fp32 SIMT kernel */
+ * 128-row tile (two m64 wgmma row blocks) with zero rows), ldg%4==0, ldx%4==0, and GY, X, in_scale and in_shift 16-byte
+ * aligned; Cin<=8 (with Cout in {32,64,128,256}, P>=4096, ldg%4==0 and GY 16-byte aligned) has an HBM-bound
+ * row-streaming kernel; otherwise the register-tiled fp32 SIMT kernel.  A precision 1 or 4 call whose shape or operands
+ * are not eligible for the wgmma kernel runs one of the fp32 kernels, without an error: its result is fp32, not TF32. */
 int usip_wgrad(const float* GY, int ldg, const float* X, int ldx, const float* in_scale, const float* in_shift,
                int in_relu, float* gW, int ldw, int P, int Cout, int Cin, int precision, void* stream);
 

@@ -6,16 +6,11 @@ import numpy as np
 import pytest
 import torch
 
+from tests.gemm_ref import tf32 as _tf32
 from tests.test_gpu_ops import _layer_ref
 from tests.util_gpu import cu, dev, rel_err
 
 pytestmark = pytest.mark.gpu
-
-
-def _tf32(a):
-    """cvt.rna.tf32.f32: round to nearest, ties away from zero, keeping 10 mantissa bits."""
-    b = np.ascontiguousarray(a, np.float32).view(np.uint32)
-    return ((b + np.uint32(0x1000)) & np.uint32(0xffffe000)).view(np.float32)
 
 
 def _run_case(P, Cin, Cout, group=0, transposed=False, single=False, add_group=0, seed=0):
