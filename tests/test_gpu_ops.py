@@ -270,12 +270,12 @@ def test_layer_fwd(P, Cin, Cout, group, precision):
 
 
 def test_bn_finalize_matches_batch_norm():
-    from usip_b200 import ops
+    from usip_b200 import _lib, ops
     P, C = 3000, 96
     torch.manual_seed(0)
     Y = torch.randn(P, C, device=dev()) * 3 + 1.5
     W = torch.eye(C, device=dev())
-    tile = ops.tile_rows(); nt = (P + tile - 1) // tile
+    tile = _lib.load().usip_layer_tile_rows(); nt = (P + tile - 1) // tile
     part = torch.zeros((nt, 2, C), device=dev())
     out = torch.empty_like(Y)
     ops.layer_fwd(Y, W, None, P, C, C, Y=out, stat_partial=part)

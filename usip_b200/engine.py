@@ -18,7 +18,6 @@ from . import _lib, ops
 
 f32 = torch.float32
 i32 = torch.int32
-EPS = 1e-5
 
 # Optional per-op device timing (bench.py): set PROFILE = {} to record CUDA-event pairs around every op of the
 # plan on the launching stream; collect_profile() turns them into mean milliseconds per op name.
@@ -56,18 +55,11 @@ def collect_profile():
     return out
 
 
-def _w2d(w):
-    """(Cout, Cin[,1[,1]]) conv weight -> [Cout, Cin] view that remembers its owning Parameter (packed-weight cache)."""
-    t = w.detach().reshape(w.shape[0], -1)
-    t._owner = w
-    return t
-
-
-def _cols(t, a, b=None):
-    """Column slice of a _w2d view (concat halves of a conv weight), keeping the owner."""
-    v = t[:, a:b]
-    v._owner = getattr(t, "_owner", None)
-    return v
+def _conv_w(layer, cols=None):
+    """[Cout, Cin] view of the conv1x1 `layer`'s weight -- only the columns `cols` (a concat half) when given -- and the
+    offset of its first column."""
+    W = layer.conv.weight.detach().flatten(1)
+    return (W, 0) if cols is None else (W[:, cols], cols.start)
 
 
 class BNState:
@@ -75,9 +67,9 @@ class BNState:
     __slots__ = ("scale", "shift", "mean", "invstd", "count")
 
 
-# Packed (hi/lo TF32, pre-swizzled) weight tiles are cached per weight view and re-used while the parameter's
-# autograd version counter is unchanged (inference / fwd-only loops); an optimizer step bumps the version and the
-# next launch re-packs into the same workspace.
+# Packed (hi/lo TF32, pre-swizzled) weight tiles are cached on the weight Parameter and re-used while its autograd
+# version counter is unchanged (inference / fwd-only loops); an optimizer step bumps the version and the next launch
+# re-packs into the same workspace.
 class _PackEntry:
     """One packed-weight workspace: the version it was packed at, and -- once the layer has run -- a copy of its descriptor,
     so that prepack_weights() can re-pack it together with all the others in one launch."""
@@ -86,25 +78,30 @@ class _PackEntry:
     def __init__(self, ver, ws, ptr):
         self.ver, self.ws, self.ptr, self.desc, self.keep, self.used_step = ver, ws, ptr, None, None, -1
 
+    def remember(self, d, W):
+        """Keep a copy of the descriptor `d` the layer launched with (its W / workspace pointers; the tensors are kept
+        alive next to it), so that the pack can join the one-launch re-pack of a train step."""
+        if self.desc is None:
+            self.desc, self.keep = ops.LayerDesc.from_buffer_copy(d), (W, self.ws)
+
 
 _PACK_STEP = [0]
 
 
-def _tc_workspace(W, P, Cin, Cout, group, transposed, prec=1):
-    """-> (workspace, already_packed, entry or None)"""
-    owner = getattr(W, "_owner", None)
-    if owner is None:                                  # unknown provenance: never reuse packed tiles
-        return torch.empty((2 * Cin * Cout,), dtype=f32, device=W.device), False, None
-    cache = owner.__dict__.setdefault("_usip_tc", {})  # lives and dies with the Parameter object
-    key = (W.data_ptr() - owner.data_ptr(), W.stride(0), P, Cin, Cout, bool(transposed), group > 32, prec)
-    ver = (owner._version, _lib.WEIGHT_GEN[0])
+def _tc_workspace(weight, col0, P, Cin, Cout, transposed):
+    """-> (workspace, already_packed, entry) of the tensor-core tiles of the conv weight Parameter `weight` as one layer
+    launch reads it: columns from col0 on, Cin x Cout as the launch sees them (swapped for a transposed use).  The key
+    holds what the pack depends on; P is there because the column-tile width follows from P and Cout."""
+    cache = weight.__dict__.setdefault("_usip_tc", {})  # lives and dies with the Parameter object
+    key = (col0, P, Cin, Cout, bool(transposed))
+    ver = (weight._version, _lib.WEIGHT_GEN[0])
     ent = cache.get(key)
-    if ent is not None and ent.ver == ver and ent.ptr == owner.data_ptr():
+    if ent is not None and ent.ver == ver and ent.ptr == weight.data_ptr():
         ent.used_step = _PACK_STEP[0]
         return ent.ws, True, ent
-    if ent is None or ent.ptr != owner.data_ptr():
-        ent = _PackEntry(ver, ent.ws if ent is not None else torch.empty((2 * Cin * Cout,), dtype=f32, device=W.device),
-                         owner.data_ptr())
+    if ent is None or ent.ptr != weight.data_ptr():
+        ent = _PackEntry(ver, ent.ws if ent is not None else torch.empty((2 * Cin * Cout,), dtype=f32, device=weight.device),
+                         weight.data_ptr())
         cache[key] = ent
     ent.ver = ver
     ent.used_step = _PACK_STEP[0]
@@ -144,7 +141,6 @@ def invalidate_packed_weights(module):
         p.__dict__.pop("_usip_tc", None)
 
 
-import os as _os
 _TC_PREC = 1          # usip_layer_desc.precision of the wgmma 3xTF32 kernel
 
 
@@ -159,12 +155,10 @@ def _precision_for(P, Cin, Cout, use_tc, group=0):
 class LayerRunner:
     """Runs conv1x1(+BN) layers of one nn.Module tree through usip_layer_fwd / usip_bn_finalize."""
 
-    def __init__(self, net, training, use_tc, dev):
-        self.net = net
+    def __init__(self, training, use_tc, dev):
         self.training = training
         self.use_tc = use_tc
         self.dev = dev
-        self.tile = ops.tile_rows()
 
     def bn_state(self, norm, part, ntiles, count, momentum):
         C = norm.weight.numel()
@@ -175,11 +169,11 @@ class LayerRunner:
         if self.training:
             st.mean = torch.empty(C, dtype=f32, device=self.dev)
             st.invstd = torch.empty(C, dtype=f32, device=self.dev)
-            ops.bn_finalize(part, ntiles, count, C, norm.weight.detach(), norm.bias.detach(), EPS, momentum,
+            ops.bn_finalize(part, ntiles, count, C, norm.weight.detach(), norm.bias.detach(), norm.eps, momentum,
                             norm.running_mean, norm.running_var, st.scale, st.shift, st.mean, st.invstd)
         else:
             st.mean = st.invstd = None
-            ops.bn_eval_affine(norm.weight.detach(), norm.bias.detach(), norm.running_mean, norm.running_var, EPS,
+            ops.bn_eval_affine(norm.weight.detach(), norm.bias.detach(), norm.running_mean, norm.running_var, norm.eps,
                                st.scale, st.shift)
         return st
 
@@ -189,12 +183,18 @@ class LayerRunner:
             return None, ntiles
         return torch.empty((ntiles, 2, Cout), dtype=f32, device=self.dev), ntiles
 
-    def run(self, X, P, W, bias, norm=None, momentum=0.1, prev=None, relu_in=None, Y=None, write_y=True,
-            addend=None, add_index=None, add_group=0, group=0, want_group=False, want_arg=False, count=None, name="layer"):
-        """Y = act(X) W^T + bias (+addend); returns (Y, BNState or None, group dict or None)."""
+    def conv(self, layer, X, P, prev=None, epoch=None, cols=None, node=False, relu_in=None, write_y=True, addend=None,
+             add_index=None, add_group=0, group=0, want_group=False, want_arg=False, name="layer"):
+        """Forward of the conv1x1 `layer` over P rows: Y = act(X) W^T + b (+addend), followed by the layer's BatchNorm when
+        it has one, its momentum scheduled by `epoch` (omitted where the reference calls the layer without it).  X is read
+        through relu(bn(.)) with the BNState `prev` of the layer that produced it, raw when prev is None; cols: the slice
+        of W's columns a concat half reads.  node=True: the per-node half of a concat, a plain GEMM (no bias, no
+        BatchNorm).  Returns (Y, BNState or None, group dict or None)."""
+        W, col0 = _conv_w(layer, cols)
+        bias = None if node else layer.conv.bias.detach()
+        norm = None if node else getattr(layer, "norm", None)
         Cout, Cin = W.shape
-        if Y is None and write_y:
-            Y = torch.empty((P, Cout), dtype=f32, device=self.dev)
+        Y = torch.empty((P, Cout), dtype=f32, device=self.dev) if write_y else None
         prec = _precision_for(P, Cin, Cout, self.use_tc, group if want_group else 0)
         part, ntiles = self.partials(P, Cout, prec, group, want_group) if norm is not None else (None, 0)
         grp = None
@@ -205,32 +205,25 @@ class LayerRunner:
             if want_arg:
                 grp["amax"] = torch.empty((Q, Cout), dtype=i32, device=self.dev)
                 grp["amin"] = torch.empty((Q, Cout), dtype=i32, device=self.dev)
-        ws, packed, pack_ent = _tc_workspace(W, P, Cin, Cout, group if want_group else 0, False, prec) if prec else (None, False, None)
+        ws, packed, ent = _tc_workspace(layer.conv.weight, col0, P, Cin, Cout, False) if prec else (None, False, None)
         with _Prof("%s[%dx%d->%d]" % (name, P, Cin, Cout), flops=2.0 * P * Cin * Cout,
                    precision="3xTF32 wgmma" if prec else "fp32 SIMT"):
-            ops.layer_fwd(X, W, bias, P, Cin, Cout,
-                          in_scale=None if prev is None else prev.scale, in_shift=None if prev is None else prev.shift,
-                          in_relu=(prev is not None) if relu_in is None else relu_in,
-                          addend=addend, add_index=add_index, add_group=add_group, Y=Y if write_y else None,
-                          stat_partial=part,
-                          gmax=None if grp is None else grp["gmax"], gmin=None if grp is None else grp["gmin"],
-                          garg_max=None if grp is None else grp.get("amax"),
-                          garg_min=None if grp is None else grp.get("amin"),
-                          group=group, precision=prec, tc_ws=ws, tc_packed=packed, pack_entry=pack_ent)
+            d = ops.layer_fwd(X, W, bias, P, Cin, Cout,
+                              in_scale=None if prev is None else prev.scale, in_shift=None if prev is None else prev.shift,
+                              in_relu=(prev is not None) if relu_in is None else relu_in,
+                              addend=addend, add_index=add_index, add_group=add_group, Y=Y,
+                              stat_partial=part,
+                              gmax=None if grp is None else grp["gmax"], gmin=None if grp is None else grp["gmin"],
+                              garg_max=None if grp is None else grp.get("amax"),
+                              garg_min=None if grp is None else grp.get("amin"),
+                              group=group, precision=prec, tc_ws=ws, tc_packed=packed)
+        if ent is not None:
+            ent.remember(d, W)
         st = None
         if norm is not None:
             with _Prof("bn_finalize"):
-                st = self.bn_state(norm, part, ntiles, P if count is None else count, momentum)
+                st = self.bn_state(norm, part, ntiles, P, norm.scheduled_momentum(epoch))
         return Y, st, grp
-
-
-def _bn_mom(norm, epoch):
-    """layers.py:62-66 -- side effect on norm.momentum kept, like the reference."""
-    if (epoch is not None) and (epoch >= 1) and (norm.momentum_decay_step is not None) and (norm.momentum_decay_step > 0):
-        norm.momentum = norm.momentum_original * (norm.momentum_decay ** (epoch // norm.momentum_decay_step))
-        if norm.momentum < 0.01:
-            norm.momentum = 0.01
-    return norm.momentum
 
 
 def _knn_head_forward(R, net, AGG, C1, coords, Bp, M, Kn, epoch, keep):
@@ -246,26 +239,24 @@ def _knn_head_forward(R, net, AGG, C1, coords, Bp, M, Kn, epoch, keep):
     ka = net.knnlayer_1.layers_after
     C2 = ka[-1].conv.weight.shape[0]
     pool2 = AGG[:, :C1]
-    cmean = coords
     # ---- GeneralKNNFusionModule (layers.py:401-440)
     with _Prof("knn_nodes"):
-        knn_i = ops.knn_nodes(cmean, Kn)
-    W5 = _w2d(kb[0].conv.weight)
+        knn_i = ops.knn_nodes(coords, Kn)
+    W5, _ = _conv_w(kb[0])
     Cb = W5.shape[0]
-    Z, _, _ = R.run(pool2, Q, _cols(W5, 3), None, relu_in=False, name="knn_b0_node")
+    Z, _, _ = R.conv(kb[0], pool2, Q, cols=slice(3, None), node=True, name="knn_b0_node")
     Y5 = torch.empty((G, Cb), dtype=f32, device=dev)
     part5, nt5 = R.partials(G, Cb)
     with _Prof("knn_combine", nbytes=8.0 * G * Cb):
-        ops.knn_combine(Z, cmean, knn_i, W5, W5.stride(0), kb[0].conv.bias.detach(), Y5, part5, Bp, M, Kn, Cb)
-    bn5 = R.bn_state(kb[0].norm, part5, nt5, G, _bn_mom(kb[0].norm, epoch))
+        ops.knn_combine(Z, coords, knn_i, W5, W5.stride(0), kb[0].conv.bias.detach(), Y5, part5, Bp, M, Kn, Cb)
+    bn5 = R.bn_state(kb[0].norm, part5, nt5, G, kb[0].norm.scheduled_momentum(epoch))
     prev, Yprev = bn5, Y5
     saved_before = [(Y5, bn5)]
     grp_b = None
     for li in range(1, len(kb)):
         last = li == len(kb) - 1
-        Yn, bnn, grp = R.run(Yprev, G, _w2d(kb[li].conv.weight), kb[li].conv.bias.detach(), kb[li].norm,
-                             _bn_mom(kb[li].norm, epoch), prev=prev, group=Kn, want_group=last, want_arg=last and keep,
-                             name="knn_b%d" % li)
+        Yn, bnn, grp = R.conv(kb[li], Yprev, G, prev=prev, epoch=epoch, group=Kn, want_group=last, want_arg=last and keep,
+                              name="knn_b%d" % li)
         prev, Yprev = bnn, Yn
         saved_before.append((Yn, bnn))
         grp_b = grp if last else grp_b
@@ -273,31 +264,27 @@ def _knn_head_forward(R, net, AGG, C1, coords, Bp, M, Kn, epoch, keep):
     amax = torch.empty((Q, Cb), dtype=f32, device=dev)
     with _Prof("group_select"):
         ops.group_select(grp_b["gmax"], grp_b["gmin"], prev.scale, prev.shift, amax, Q, Cb)
-    W8 = _w2d(ka[0].conv.weight)
-    U, _, _ = R.run(amax, Q, _cols(W8, 0, Cb), None, relu_in=False, name="knn_a0_node")                                    # max half (layers.py:435)
-    Y8, bn8, _ = R.run(Yprev, G, _cols(W8, Cb), ka[0].conv.bias.detach(), ka[0].norm, _bn_mom(ka[0].norm, epoch),
-                       prev=prev, addend=U, add_group=Kn, name="knn_a0")
+    U, _, _ = R.conv(ka[0], amax, Q, cols=slice(0, Cb), node=True, name="knn_a0_node")        # max half (layers.py:435)
+    Y8, bn8, _ = R.conv(ka[0], Yprev, G, prev=prev, epoch=epoch, cols=slice(Cb, None), addend=U, add_group=Kn,
+                        name="knn_a0")
     saved_after = [(Y8, bn8)]
     prevA, YA = bn8, Y8
     grp_a = None
     for li in range(1, len(ka)):
         last = li == len(ka) - 1
-        Yn, bnn, grp = R.run(YA, G, _w2d(ka[li].conv.weight), ka[li].conv.bias.detach(), ka[li].norm,
-                             _bn_mom(ka[li].norm, epoch), prev=prevA, group=Kn, want_group=last, want_arg=last and keep,
-                             write_y=(not last) or keep, name="knn_a%d" % li)
+        Yn, bnn, grp = R.conv(ka[li], YA, G, prev=prevA, epoch=epoch, group=Kn, want_group=last, want_arg=last and keep,
+                              write_y=(not last) or keep, name="knn_a%d" % li)
         prevA, YA = bnn, Yn
         saved_after.append((Yn, bnn))
         grp_a = grp if last else grp_a
     ops.group_select(grp_a["gmax"], grp_a["gmin"], prevA.scale, prevA.shift, AGG[:, C1:], Q, C2)   # layers.py:438
 
     # ---- head (networks.py:143-154); mlp1/mlp2 are called WITHOUT epoch in the reference
-    Y10, bn10, _ = R.run(AGG, Q, _w2d(net.mlp1.conv.weight), net.mlp1.conv.bias.detach(), net.mlp1.norm,
-                         net.mlp1.norm.momentum, relu_in=False, name="mlp1")
-    Y11, bn11, _ = R.run(Y10, Q, _w2d(net.mlp2.conv.weight), net.mlp2.conv.bias.detach(), net.mlp2.norm,
-                         net.mlp2.norm.momentum, prev=bn10, name="mlp2")
-    OUT, _, _ = R.run(Y11, Q, _w2d(net.mlp3.conv.weight), net.mlp3.conv.bias.detach(), prev=bn11, name="mlp3")
+    Y10, bn10, _ = R.conv(net.mlp1, AGG, Q, name="mlp1")
+    Y11, bn11, _ = R.conv(net.mlp2, Y10, Q, prev=bn10, name="mlp2")
+    OUT, _, _ = R.conv(net.mlp3, Y11, Q, prev=bn11, name="mlp3")
     with _Prof("head_finalize"):
-        keypoints, sigmas = ops.head_finalize(OUT, cmean, opt.loss_sigma_lower_bound, Bp, M)
+        keypoints, sigmas = ops.head_finalize(OUT, coords, opt.loss_sigma_lower_bound, Bp, M)
 
     kctx = dict(knn_i=knn_i)
     if keep:
@@ -326,7 +313,7 @@ def detector_forward(net, x, sn, node, epoch=None, use_tc=True, keep=False):
     P, Q = Bp * N, Bp * M
     G = Q * Kn
     training = net.training
-    R = LayerRunner(net, training, use_tc, dev)
+    R = LayerRunner(training, use_tc, dev)
     x = x.detach().contiguous(); node = node.detach().contiguous()
     snc = sn.detach().contiguous() if S else None
 
@@ -341,20 +328,18 @@ def detector_forward(net, x, sn, node, epoch=None, use_tc=True, keep=False):
     # ---- first PointNet (3+S -> C1/2 -> C1/2 -> C1/2), networks.py:111-114
     fp = net.first_pointnet.layers
     H = fp[0].conv.weight.shape[0]
-    Y0, bn0, _ = R.run(X0, P, _w2d(fp[0].conv.weight), fp[0].conv.bias.detach(), fp[0].norm, _bn_mom(fp[0].norm, epoch), name="pn1.0")
-    Y1, bn1, _ = R.run(Y0, P, _w2d(fp[1].conv.weight), fp[1].conv.bias.detach(), fp[1].norm, _bn_mom(fp[1].norm, epoch), prev=bn0, name="pn1.1")
-    F1, _, _ = R.run(Y1, P, _w2d(fp[2].conv.weight), fp[2].conv.bias.detach(), prev=bn1, name="pn1.2")
+    Y0, bn0, _ = R.conv(fp[0], X0, P, epoch=epoch, name="pn1.0")
+    Y1, bn1, _ = R.conv(fp[1], Y0, P, prev=bn0, epoch=epoch, name="pn1.1")
+    F1, _, _ = R.conv(fp[2], Y1, P, prev=bn1, name="pn1.2")
     # ---- pool 1 (index_max + gather * mask, networks.py:117-120)
     with _Prof("segmax1", nbytes=4.0 * P * H):
         pool1, arg1 = ops.segmax(F1, H, seg_off, perm, Bp, N, M, want_arg=keep)
     # ---- second PointNet on cat(first, scattered max) (networks.py:123-127): W [f; s] = Wa f + Wb s
     sp = net.second_pointnet.layers
     C1 = sp[0].conv.weight.shape[0]
-    W3 = _w2d(sp[0].conv.weight)
-    V, _, _ = R.run(pool1, Q, _cols(W3, H), None, relu_in=False, name="pn2.0_node")
-    Y3, bn3, _ = R.run(F1, P, _cols(W3, 0, H), sp[0].conv.bias.detach(), sp[0].norm, _bn_mom(sp[0].norm, epoch),
-                       relu_in=False, addend=V, add_index=row_seg, name="pn2.0")
-    F2, _, _ = R.run(Y3, P, _w2d(sp[1].conv.weight), sp[1].conv.bias.detach(), prev=bn3, name="pn2.1")
+    V, _, _ = R.conv(sp[0], pool1, Q, cols=slice(H, None), node=True, name="pn2.0_node")
+    Y3, bn3, _ = R.conv(sp[0], F1, P, epoch=epoch, cols=slice(0, H), addend=V, add_index=row_seg, name="pn2.0")
+    F2, _, _ = R.conv(sp[1], Y3, P, prev=bn3, name="pn2.1")
     # ---- pool 2 -> first C1 columns of the head input (networks.py:130-133,143)
     C2 = net.knnlayer_1.layers_after[-1].conv.weight.shape[0]
     AGG = torch.empty((Q, C1 + C2), dtype=f32, device=dev)
@@ -390,7 +375,6 @@ class _Bwd:
     """Small helper bundle for the backward plans: raw C-ABI calls + gradient bookkeeping."""
 
     def __init__(self, net, dev, use_tc):
-        from . import _lib
         self.lib = _lib.load()
         self.check = _lib.check
         self.dev = dev
@@ -475,17 +459,20 @@ class _Bwd:
                                            None if prev is None else p(prev.shift), 1 if (relu or prev is not None) else 0,
                                            p(gW), gW.stride(0), P, Cout, Cin, (4 if self.tf32_bwd else 1) if self.use_tc else 0, s), "usip_wgrad")
 
-    def dgrad(self, GY, W2d, P, name="dgrad", out=None):
-        """G_in[P,Cin] = GY[P,Cout] @ W2d[Cout,Cin] (the forward weight, used transposed by the layer kernel)."""
+    def dgrad(self, GY, layer, P, cols=None, name="dgrad"):
+        """G_in[P,Cin] = GY[P,Cout] @ W[Cout,Cin], W the forward weight of the conv1x1 `layer` (its columns `cols` when
+        given), used transposed by the layer kernel."""
+        W2d, col0 = _conv_w(layer, cols)
         Cout, Cin = W2d.shape
-        if out is None:
-            out = torch.empty((P, Cin), dtype=f32, device=self.dev)
+        out = torch.empty((P, Cin), dtype=f32, device=self.dev)
         prec = _precision_for(P, Cout, Cin, self.use_tc)
-        ws, packed, pack_ent = _tc_workspace(W2d, P, Cout, Cin, 0, True, prec) if prec else (None, False, None)
+        ws, packed, ent = _tc_workspace(layer.conv.weight, col0, P, Cout, Cin, True) if prec else (None, False, None)
         with _Prof("%s[%dx%d->%d]" % (name, P, Cout, Cin), flops=2.0 * P * Cin * Cout,
                    precision="3xTF32 wgmma" if prec else "fp32 SIMT"):
-            ops.layer_fwd(GY, W2d, None, P, Cout, Cin, Y=out, precision=prec, w_transposed=True, tc_ws=ws, tc_packed=packed,
-                          debug_flags=8 if (self.tf32_bwd and prec) else 0, pack_entry=pack_ent)
+            d = ops.layer_fwd(GY, W2d, None, P, Cout, Cin, Y=out, precision=prec, w_transposed=True, tc_ws=ws, tc_packed=packed,
+                              debug_flags=8 if (self.tf32_bwd and prec) else 0)
+        if ent is not None:
+            ent.remember(d, W2d)
         return out
 
     def colsum(self, G, out, P, C):
@@ -498,10 +485,10 @@ class _Bwd:
         Accumulates the weight (and bias) gradient and returns the gradient of act(X) -- or, given the input layer's
         BatchNorm `norm`, of that layer's pre-BN output (profile record "bn_bwd_<in_name>"); GY is consumed then, its buffer
         released before bn_bwd allocates the next one.  grad_in=False (a plan's first layer): the weight gradient only."""
-        W, gW = _w2d(layer.conv.weight), self.g2d(layer.conv.weight)
+        gW = self.g2d(layer.conv.weight)
         if cols is not None:
-            W, gW = _cols(W, cols.start, cols.stop), gW[:, cols]
-        Cout, Cin = W.shape
+            gW = gW[:, cols]
+        Cout, Cin = gW.shape
         self.wgrad(GY, X, gW, P, Cout, Cin, prev=prev, name="wgrad_" + name)
         # a conv bias in front of a train-mode BatchNorm receives exactly zero gradient (BN removes the mean): it stays
         # zero-initialised in self.grads
@@ -509,7 +496,7 @@ class _Bwd:
             self.colsum(GY, self.grads[layer.conv.bias], P, Cout)
         if not grad_in:
             return None
-        G_in = self.dgrad(GY, W, P, name="dgrad_" + name)
+        G_in = self.dgrad(GY, layer, P, cols, name="dgrad_" + name)
         if norm is None:
             return G_in
         GY.set_()                                   # frees GY's buffer even though the caller still holds the tensor
@@ -638,23 +625,19 @@ def _group_net_forward(R, net, rows, Bp, M, K, keep, out=None):
         raise NotImplementedError("group of %d rows: groups above 128 must be a multiple of 64" % K)
     c1, c2, c3, c4, c5 = net.conv1, net.conv2, net.conv3, net.conv4, net.conv5
     D = c3.conv.weight.shape[0]
-    Y1, bn1, _ = R.run(rows, G, _w2d(c1.conv.weight), c1.conv.bias.detach(), c1.norm, c1.norm.momentum, name="grp.conv1")
-    Y2, bn2, _ = R.run(Y1, G, _w2d(c2.conv.weight), c2.conv.bias.detach(), c2.norm, c2.norm.momentum, prev=bn1, name="grp.conv2")
-    Y3, bn3, grp3 = R.run(Y2, G, _w2d(c3.conv.weight), c3.conv.bias.detach(), c3.norm, c3.norm.momentum, prev=bn2,
-                          group=sub, want_group=True, want_arg=keep, name="grp.conv3")
+    Y1, bn1, _ = R.conv(c1, rows, G, name="grp.conv1")
+    Y2, bn2, _ = R.conv(c2, Y1, G, prev=bn1, name="grp.conv2")
+    Y3, bn3, grp3 = R.conv(c3, Y2, G, prev=bn2, group=sub, want_group=True, want_arg=keep, name="grp.conv3")
     if sub != K:
         _combine_sub_groups(grp3, K // sub, sub, keep)
     amax = torch.empty((Q, D), dtype=f32, device=dev)
     ops.group_select(grp3["gmax"], grp3["gmin"], bn3.scale, bn3.shift, amax, Q, D)          # y_first_max (networks.py:377)
-    W4 = _w2d(c4.conv.weight)
-    C4 = W4.shape[0]
-    U, _, _ = R.run(amax, Q, _cols(W4, D), None, relu_in=False, name="grp.conv4_node")        # cat(y_first, max): max is LAST
-    Y4, bn4, _ = R.run(Y3, G, _cols(W4, 0, D), c4.conv.bias.detach(), c4.norm, c4.norm.momentum, prev=bn3, addend=U,
-                       add_group=K, name="grp.conv4")
+    C4 = c4.conv.weight.shape[0]
+    U, _, _ = R.conv(c4, amax, Q, cols=slice(D, None), node=True, name="grp.conv4_node")   # cat(y_first, max): max is LAST
+    Y4, bn4, _ = R.conv(c4, Y3, G, prev=bn3, cols=slice(0, D), addend=U, add_group=K, name="grp.conv4")
     last_bn = getattr(c5, "norm", None) is not None
-    Y5, bn5, grp5 = R.run(Y4, G, _w2d(c5.conv.weight), c5.conv.bias.detach(), c5.norm if last_bn else None,
-                          c5.norm.momentum if last_bn else 0.1, prev=bn4, group=sub, want_group=True, want_arg=keep,
-                          write_y=last_bn and keep, name="grp.conv5")
+    Y5, bn5, grp5 = R.conv(c5, Y4, G, prev=bn4, group=sub, want_group=True, want_arg=keep, write_y=last_bn and keep,
+                           name="grp.conv5")
     if sub != K:
         if not last_bn:                                    # a linear conv5 is pooled by its max only
             grp5["gmin"] = grp5["amin"] = None
@@ -693,7 +676,7 @@ def ablation_forward(net, x, sn, node, epoch=None, use_tc=True, keep=False, mode
     Kn = opt.node_knn_k_1
     K = ABLATION_K
     Q = Bp * M
-    R = LayerRunner(net, net.training, use_tc, dev)
+    R = LayerRunner(net.training, use_tc, dev)
     x = x.detach().contiguous(); node = node.detach().contiguous()
     snc = sn.detach().contiguous() if S else None
     with _Prof("group_%s" % mode):
@@ -729,14 +712,13 @@ def ablation_backward(net, ctx, g_kp, g_sig):
 def descriptor_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=True, keep=False):
     """DescriptorLiteOld.forward (models/networks.py:333-385) on the fused plan.
     Returns (descriptor (B,C,M), x_features (B,3+S,M,K), ctx) -- ctx holds what descriptor_backward needs (keep=True)."""
-    from . import _lib
     opt = net.opt
     dev = x.device
     if keep and not net.training:
         raise NotImplementedError("gradients through eval-mode BatchNorm are not part of the hot path "
                                   "(the reference only back-propagates in train mode, keypoint_descriptor.py:138)")
     Bp, M, K = x.shape[0], keypoints.shape[2], opt.ball_nsamples
-    R = LayerRunner(net, net.training, use_tc, dev)
+    R = LayerRunner(net.training, use_tc, dev)
     feats, rows = _descriptor_balls(opt, x, sn, keypoints, permute_idx)
     gmax5, gctx = _group_net_forward(R, net, rows, Bp, M, K, keep, out=None)
     D = gctx["D"]
@@ -781,7 +763,7 @@ def descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=
                                   "(the reference only back-propagates in train mode, keypoint_descriptor.py:466)")
     Bp, M, K = x.shape[0], keypoints.shape[2], opt.ball_nsamples
     Q = Bp * M
-    R = LayerRunner(net, net.training, use_tc, dev)
+    R = LayerRunner(net.training, use_tc, dev)
     feats, rows = _descriptor_balls(opt, x, sn, keypoints, permute_idx)
     local, gctx = _group_net_forward(R, net, rows, Bp, M, K, keep, out=None)         # [Q, D] raw max of conv5
     D = gctx["D"]
@@ -791,12 +773,10 @@ def descriptor_global_forward(net, x, sn, keypoints, epoch, permute_idx, use_tc=
         else:
             glob, _ = ops.group_max_combine(local, M)
     f1, f2, f3 = net.fc1, net.fc2, net.fc3
-    W1 = _w2d(f1.conv.weight)
-    U, _, _ = R.run(glob, Bp, _cols(W1, D), None, relu_in=False, name="fc1_global")   # cat(desc, global): global is LAST
-    Y1, bn1, _ = R.run(local, Q, _cols(W1, 0, D), f1.conv.bias.detach(), f1.norm, f1.norm.momentum, relu_in=False,
-                       addend=U, add_group=M, name="fc1")
-    Y2, bn2, _ = R.run(Y1, Q, _w2d(f2.conv.weight), f2.conv.bias.detach(), f2.norm, f2.norm.momentum, prev=bn1, name="fc2")
-    OUT, _, _ = R.run(Y2, Q, _w2d(f3.conv.weight), f3.conv.bias.detach(), prev=bn2, name="fc3")
+    U, _, _ = R.conv(f1, glob, Bp, cols=slice(D, None), node=True, name="fc1_global")   # cat(desc, global): global is LAST
+    Y1, bn1, _ = R.conv(f1, local, Q, cols=slice(0, D), addend=U, add_group=M, name="fc1")
+    Y2, bn2, _ = R.conv(f2, Y1, Q, prev=bn1, name="fc2")
+    OUT, _, _ = R.conv(f3, Y2, Q, prev=bn2, name="fc3")
     desc = torch.empty((Bp, OUT.shape[1], M), dtype=f32, device=dev)
     _lib.check(_lib.load().usip_l2norm_to_bcm(ops._p(OUT), OUT.stride(0), ops._p(desc), None, Bp, M, OUT.shape[1],
                                               ops._stream()), "usip_l2norm_to_bcm")

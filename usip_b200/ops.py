@@ -30,10 +30,6 @@ def _req(t, dtype, name):
         raise RuntimeError("%s: expected dtype %s, got %s" % (name, dtype, t.dtype))
 
 
-def tile_rows():
-    return _lib.load().usip_layer_tile_rows()
-
-
 def stat_slots(P, Cout, precision=0, group=0, want_group=False):
     """Rows of the [slots, 2, Cout] BN-statistic partial buffer usip_layer_fwd fills for this layer shape."""
     d = _lib.LayerDesc()
@@ -682,8 +678,8 @@ def knn_nodes(pts, K):
 # ----------------------------------------------------------------------------- shared-MLP stack
 def layer_fwd(X, W, bias, P, Cin, Cout, ldx=None, ldw=None, in_scale=None, in_shift=None, in_relu=False,
               addend=None, add_index=None, add_group=0, Y=None, ldy=None, stat_partial=None,
-              gmax=None, gmin=None, garg_max=None, garg_min=None, group=0, precision=0, tc_ws=None, tc_packed=False, w_transposed=False, debug_flags=0, debug_clocks=None,
-              pack_entry=None):
+              gmax=None, gmin=None, garg_max=None, garg_min=None, group=0, precision=0, tc_ws=None, tc_packed=False, w_transposed=False, debug_flags=0, debug_clocks=None):
+    """Launches one layer; returns the LayerDesc it launched with."""
     d = LayerDesc()
     d.X = X.data_ptr(); d.ldx = X.stride(0) if ldx is None else ldx
     d.P = P; d.Cin = Cin; d.Cout = Cout
@@ -713,13 +709,9 @@ def layer_fwd(X, W, bias, P, Cin, Cout, ldx=None, ldw=None, in_scale=None, in_sh
             tc_ws = torch.empty((2 * Cin * Cout,), dtype=f32, device=X.device)
         d.tc_workspace = tc_ws.data_ptr(); d.tc_workspace_bytes = tc_ws.numel() * 4
         d.tc_weights_packed = 1 if tc_packed else 0
-        if pack_entry is not None and pack_entry.desc is None:
-            # remembered for engine.prepack_weights(): the pack of this layer can then join the one-launch re-pack of a
-            # train step (the copy keeps W / workspace pointers; the tensors are kept alive next to it)
-            pack_entry.desc = LayerDesc.from_buffer_copy(d)
-            pack_entry.keep = (W, tc_ws)
     check(_lib.load().usip_layer_fwd(ctypes.byref(d), _stream()),
           "usip_layer_fwd_tc" if (precision == 1 and not tc_packed) else "usip_layer_fwd")
+    return d
 
 
 def bn_finalize(stat_partial, ntiles, count, C, gamma, beta, eps, momentum, running_mean, running_var,
