@@ -331,6 +331,70 @@ int usip_ransac_info_f64(const float* xyz, const int32_t* count, int n_scans, in
                          const int32_t* trials, int nT, double threshold, uint64_t seed, const double* uniforms,
                          const int32_t* best_trial, const int32_t* status, double* info, int32_t* n_info, void* stream);
 
+/* Fast Global Registration    evaluation/matlab/eval_indoor/fgr/ (fast_global_registration.cpp, register2FragmentsFGR.m):
+ * FGR (Zhou, Park and Koltun, ECCV 2016) as the shipped mex runs it -- LoadFeature(pts1, feat1), LoadFeature(pts2,
+ * feat2), NormalizePoints(), AdvancedMatching(), OptimizePairwise(true, 640), GetOutputTrans() -- for every pair and
+ * every K of a keypoint-count sweep, one CTA per (pair, K) in one launch.  The model is x1 = R x2 + t, as
+ * usip_ransac_rt_f64's.  The FGR library's own sources are not in the reference tree; the constants below were read
+ * from the compiled fast_global_registration.mexa64: 640 iterations (mov $0x280 before the OptimizePairwise call), GNC
+ * factor 1.4 and stop scale 0.05 (f64, relative units), start scale 1.0 (GlobalScale = the max centred norm), tuple
+ * similarity 0.95f (mulss / divss), 100 * ncorr tuple trials (imul $0x64), at most 10000 tuples (cmpl $0x270f / jg)
+ * and at least 10 correspondences (cmp $0x9).  They differ from the FGR release defaults (64, 1000, 0.025).
+ *
+ * usip_desc_match_mutual_f64: the arguments of usip_desc_match_f64 without k, and its anchor / positive sets, d^2, tie
+ * and NaN rules (the same kernel, a mutual mode of its k = 1 path).  (i, j) is a match iff j is anchor i's nearest
+ * positive and i is positive j's nearest anchor; matches in ascending i.  FGR's swap of the larger fragment to the
+ * front does not change this set.  -> matches (P, nK, L, 2) i32 (anchor row, positive row), n_matches (P, nK) i32.
+ * The limits and refusals of usip_desc_match_f64.
+ *
+ * usip_fgr_f64: xyz (n_scans, L, 3) f32, count, pairs and ks as usip_desc_match_f64 (no frames: the rows are used as
+ * stored); matches / n_matches (P, nK, cap, 2) / (P, nK) i32 of usip_desc_match_mutual_f64 (cap = L there; 1 <= cap <=
+ * USIP_REG_MAX_KEYPOINTS); threshold > 0 (register2FragmentsFGR.m's inlierThreshold 0.2).  Per (pair, K), fragment 1
+ * is the anchor scan's rows 0..n1-1, n1 = min(K, count, L), fragment 2 the positive scan's n2 rows, and the
+ * correspondences are the n = min(n_matches, cap) matches in list order.  All fp64 on the f32 inputs, no contraction:
+ *   1. Normalise: mean_f = (((0 + x_0) + x_1) + ...) / max(n_f, 1) per coordinate, rows in order; scale = the max over
+ *      both fragments' rows of sqrt((x^2 + y^2) + z^2) of the centred row; normalised = (x - mean) / scale.  A scale
+ *      that is 0 or not finite (any non-finite centred norm) -> status 4, Rt = [I | mean1 - mean2].
+ *   2. Tuples: trial t = 0 .. 100 n - 1 (none when n < 3) takes the first three words w_i of Philox4x32-10 with counter
+ *      (t, 0, 0x46475254 "FGRT", 0) and key (seed lo, seed hi); index_i = min(floor((w_i 2^-32) n), n - 1), with
+ *      replacement (as rand() % n).  Edges li_k = |p_{i_k} - p_{i_{k+1 mod 3}}| of the normalised fragment-1 points,
+ *      lj_k likewise on fragment 2, each sqrt((dx^2 + dy^2) + dz^2); accepted iff li_k s < lj_k and lj_k < li_k / s for
+ *      k = 0, 1, 2, s = (double)0.95f, strictly (a repeated index gives a zero edge and is rejected).  The first 10000
+ *      accepted trials in trial order are kept (n_tuples); multiplicity[m] = the times match m appears in them.
+ *   3. GNC (OptimizePairwise): if 3 n_tuples < 10, no iterations, status 1.  Else par = 1, T = I, and for itr = 0..639:
+ *      if itr % 4 == 0 and par > 0.05, par = par / 1.4.  The sums run over the matches with a non-zero multiplicity in
+ *      ascending order (the "used" list).  For one with multiplicity w, p its normalised fragment-1 point, q its current
+ *      fragment-2 point: r = p - q, rr = (rx rx + ry ry) + rz rz, u = par / (rr + par), ws = w (u u); Jacobian rows
+ *      Jx = (0, -qz, qy, -1, 0, 0), Jy = (qz, 0, -qx, 0, -1, 0), Jz = (-qy, qx, 0, 0, 0, -1); term (a, b), a <= b, of
+ *      J^T J = ((Jx_a Jx_b + Jy_a Jy_b) + Jz_a Jz_b) ws, 21 of them row-major over the upper triangle, then the six of
+ *      J^T r = ((Jx_a rx + Jy_a ry) + Jz_a rz) ws.  Reduction of each of the 27: thread t of 256 sums used entries t,
+ *      t + 256, ... from 0.0 in that order; each warp of 32 then adds butterfly-wise, v += shfl_xor(v, o) for o = 16,
+ *      8, 4, 2, 1 (lane 0's value); then ((w_0 + w_1) + ...) + w_7 over the 8 warps.  Solve: Cholesky A = L L^T,
+ *      column j ascending: v = A_jj - L_j0^2 - ... - L_j(j-1)^2 (subtractions in k order), L_jj = sqrt(v), L_ij = (A_ij -
+ *      sum_k L_ik L_jk) / L_jj likewise; forward y_i = (-(J^T r)_i - sum_k<i L_ik y_k) / L_ii; back xi_i = (y_i -
+ *      sum_k>i L_ki xi_k) / L_ii, i descending, k ascending.  A pivot v <= 0 or not finite stops the loop with the T
+ *      reached (status 2).  delta = [Rz(xi2) Ry(xi1) Rx(xi0) | xi3, xi4, xi5] with R00 = cz cy, R01 = (cz sy) sx - sz cx,
+ *      R02 = (cz sy) cx + sz sx, R10 = sz cy, R11 = (sz sy) sx + cz cx, R12 = (sz sy) cx - cz sx, R20 = -sy, R21 = cy sx,
+ *      R22 = cy cx; T = delta T, entry (r, c) ((D_r0 T_0c + D_r1 T_1c) + D_r2 T_2c) (+ D_r3 in column 3); every used q
+ *      moves to ((D_r0 qx + D_r1 qy) + D_r2 qz) + D_r3.  sin and cos are CUDA's, the only steps not correctly rounded.
+ *   4. GetOutputTrans: R = T[:, :3]; t_r = ((-((R_r0 m2x + R_r1 m2y) + R_r2 m2z)) + T_r3 scale) + mean1_r; with no
+ *      iterations (status 1) and for status 4 this is [I | mean1 - mean2].
+ *   Statistics (our addition; register2FragmentsFGR.m writes constants): under the final Rt, the inliers are the matches
+ *   with sqrt((dx^2 + dy^2) + dz^2) < threshold, as usip_ransac_rt_f64's test, and info = the sum over them in match
+ *   order of usip_ransac_info_f64's A^T A at the raw fragment-1 point.  A match index outside rows 0..n1-1 / 0..n2-1:
+ *   status 3, Rt, info and counts zero.
+ *   The library seeds rand() with time(NULL) and runs FLANN and its point updates in float; here the stream is keyed
+ *   by the seed (the same for every pair and K) and every step is fp64.  The library divides by zero for ncorr = 0;
+ *   here that is status 1.
+ * -> Rt (P, nK, 3, 4) f64, n_tuples, n_inliers, status (P, nK) i32 (0 ok, 1 fewer than 10 correspondences, 2 singular
+ *    solve, 3 bad match index, 4 degenerate scale), info (P, nK, 6, 6) f64 row-major. */
+int usip_desc_match_mutual_f64(const float* desc, const int32_t* count, int n_scans, int L, int D, const int32_t* pairs,
+                               int P, const int32_t* ks, int nK, int32_t* matches, int32_t* n_matches, void* stream);
+int usip_fgr_f64(const float* xyz, const int32_t* count, int n_scans, int L, const int32_t* pairs, int P,
+                 const int32_t* ks, int nK, const int32_t* matches, const int32_t* n_matches, int cap, uint64_t seed,
+                 double threshold, double* Rt, int32_t* n_tuples, int32_t* n_inliers, double* info, int32_t* status,
+                 void* stream);
+
 /* Fragment overlap      register2Fragments.m:134-137 (ratioAligned(1)), for J (fragment a, fragment b, map) jobs at once.
  * xyz (sum of rows, 3) f32: every fragment's rows packed (columns 0:3 of its .npy), device; offsets (n_frags + 1) i64,
  * HOST memory, offsets[0] = 0, fragment f = rows [offsets[f], offsets[f+1]); jobs (J, 2) i32, HOST memory: fragment a

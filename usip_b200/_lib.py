@@ -96,6 +96,10 @@ SIGNATURES = {
     "usip_ransac_uniforms": (c_int, [ctypes.c_uint64, c_int, c_ptr, c_ptr]),
     "usip_ransac_info_f64": (c_int, [c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_int, c_ptr, c_ptr, c_int, c_ptr,
                                      c_int, ctypes.c_double, ctypes.c_uint64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr]),
+    "usip_desc_match_mutual_f64": (c_int, [c_ptr, c_ptr, c_int, c_int, c_int, c_ptr, c_int, c_ptr, c_int, c_ptr, c_ptr,
+                                           c_ptr]),
+    "usip_fgr_f64": (c_int, [c_ptr, c_ptr, c_int, c_int, c_ptr, c_int, c_ptr, c_int, c_ptr, c_ptr, c_int, ctypes.c_uint64,
+                             ctypes.c_double, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr]),
     "usip_fragment_overlap_scratch_bytes": (ctypes.c_size_t, [c_i64, c_int, c_int]),
     "usip_fragment_overlap_f32": (c_int, [c_ptr, c_ptr, c_int, c_ptr, c_ptr, c_int, c_f32, c_ptr, ctypes.c_size_t, c_ptr,
                                           c_ptr]),

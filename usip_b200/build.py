@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_DIR = os.path.join(_HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libusip_b200.so")
-SOURCES = ["api.cu", "group.cu", "indexmax.cu", "ballquery.cu", "ballgroup.cu", "knngroup.cu", "loss.cu", "nngrid.cu", "mlp.cu", "mlp_tc.cu", "backward.cu", "wgrad_tc.cu", "fps.cu", "pairgen.cu", "repeatability.cu", "registration.cu", "overlap.cu", "nms.cu", "optim.cu", "handcrafted.cu"]
+SOURCES = ["api.cu", "group.cu", "indexmax.cu", "ballquery.cu", "ballgroup.cu", "knngroup.cu", "loss.cu", "nngrid.cu", "mlp.cu", "mlp_tc.cu", "backward.cu", "wgrad_tc.cu", "fps.cu", "pairgen.cu", "repeatability.cu", "registration.cu", "fgr.cu", "overlap.cu", "nms.cu", "optim.cu", "handcrafted.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

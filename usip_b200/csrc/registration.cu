@@ -5,7 +5,7 @@
 // Arithmetic: fp64 with a fixed order and no contraction (__dadd_rn / __dmul_rn / __ddiv_rn / __dsqrt_rn), so that a
 // float64 restatement on the host (tests/reg_ref.py) reproduces every match, every hypothesis and every stop.  The
 // only transcendental that decides anything is the log of ransac.m's trial estimate N; see the header.
-#include "common.cuh"
+#include "registration.cuh"
 
 namespace usip {
 
@@ -13,10 +13,7 @@ constexpr int REG_THREADS = 256;          // also the RANSAC chunk: hypotheses e
 constexpr int REG_JACOBI_SWEEPS = 8;
 constexpr uint32_t REG_PHILOX_TAG = 0x52414e53u;
 
-struct RegKs { int32_t k[USIP_REP_MAX_K]; };
 struct RegTrials { int32_t t[USIP_REG_MAX_SWEEP]; };
-
-__device__ __forceinline__ double dsub(double a, double b) { return __dadd_rn(a, -b); }
 
 // ------------------------------------------------------------------------------------------------ matching
 // Top-k of one query row against rows 0..n-1 of `set` (both (., D) f32), ordered by (d^2, index); d^2 is
@@ -50,7 +47,9 @@ __device__ int reg_topk(const float* __restrict__ q, const float* __restrict__ s
   return min(k, n);
 }
 
-// one CTA per (pair, K).  smem (k > 1): an na x np bitset of the union and the per-row counts.
+// one CTA per (pair, K).  smem (k > 1): an na x np bitset of the union and the per-row counts.  MUTUAL (k == 1): each
+// side's 1-NN (2 L ints), intersected: (i, j) is kept iff j is i's nearest and i is j's nearest, in ascending i.
+template <bool MUTUAL>
 __global__ void __launch_bounds__(REG_THREADS)
 desc_match_kernel(const float* __restrict__ desc, const int32_t* __restrict__ count, int L, int D,
                   const int32_t* __restrict__ pairs, RegKs ks, int nK, int k, int cap, int32_t* __restrict__ matches,
@@ -64,6 +63,32 @@ desc_match_kernel(const float* __restrict__ desc, const int32_t* __restrict__ co
   const float* Q = desc + (int64_t)sp * L * D;
   int32_t* out = matches + ((int64_t)p * nK + kk) * cap * 2;
   int best[8];
+
+  if constexpr (MUTUAL) {
+    int32_t* nn_a = (int32_t*)match_smem;                       // na: anchor i's nearest positive
+    int32_t* nn_p = nn_a + L;                                   // np: positive j's nearest anchor
+    __shared__ int warp_tot[REG_THREADS / 32];
+    for (int i = tid; i < na; i += blockDim.x) {
+      reg_topk<1>(A + (int64_t)i * D, Q, np, D, 1, best);
+      nn_a[i] = best[0];
+    }
+    for (int j = tid; j < np; j += blockDim.x) {
+      reg_topk<1>(Q + (int64_t)j * D, A, na, D, 1, best);
+      nn_p[j] = best[0];
+    }
+    __syncthreads();
+    int n = 0;
+    for (int base = 0; base < na; base += blockDim.x) {         // every thread runs every round: the rank has barriers
+      const int i = base + tid;
+      const bool keep = i < na && np > 0 && nn_p[nn_a[i]] == i;
+      int total;
+      const int at = n + reg_block_rank(keep, warp_tot, &total);
+      if (keep) { out[2 * at] = i; out[2 * at + 1] = nn_a[i]; }
+      n += total;
+    }
+    if (tid == 0) n_matches[(int64_t)p * nK + kk] = n;
+    return;
+  }
 
   if (k == 1) {
     for (int i = tid; i < na; i += blockDim.x) {
@@ -276,16 +301,6 @@ __device__ __forceinline__ void reg_fit3(const double (*x)[3], const double (*y)
   reg_horn_finish(B, xb, yb, Rt);
 }
 
-// ||x1 - (R x2 + t)|| < thr, each row ((R0 x + R1 y) + R2 z) + t, then ((dx^2 + dy^2) + dz^2), sqrt
-__device__ __forceinline__ bool reg_inlier(const double* Rt, double ax, double ay, double az, double px, double py,
-                                           double pz, double thr) {
-  const double ex = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(Rt[0], px), __dmul_rn(Rt[1], py)), __dmul_rn(Rt[2], pz)), Rt[3]);
-  const double ey = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(Rt[4], px), __dmul_rn(Rt[5], py)), __dmul_rn(Rt[6], pz)), Rt[7]);
-  const double ez = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(Rt[8], px), __dmul_rn(Rt[9], py)), __dmul_rn(Rt[10], pz)), Rt[11]);
-  const double dx = dsub(ax, ex), dy = dsub(ay, ey), dz = dsub(az, ez);
-  return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz))) < thr;
-}
-
 struct RegShared {                          // the static part of the RANSAC kernel's shared memory
   int32_t cnt[REG_THREADS];
   double Rt[12];
@@ -490,14 +505,6 @@ ransac_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ count, 
   }
 }
 
-// Column k of register2Fragments.m's A = [I3 | [[0, 2z, -2y], [-2z, 0, 2x], [2y, -2x, 0]]] at (x, y, z)
-__device__ __forceinline__ void reg_info_col(int k, double x, double y, double z, double a[3]) {
-  const double x2 = __dmul_rn(2.0, x), y2 = __dmul_rn(2.0, y), z2 = __dmul_rn(2.0, z);
-  a[0] = k == 0 ? 1.0 : k == 4 ? z2 : k == 5 ? -y2 : 0.0;
-  a[1] = k == 1 ? 1.0 : k == 3 ? -z2 : k == 5 ? x2 : 0.0;
-  a[2] = k == 2 ? 1.0 : k == 3 ? y2 : k == 4 ? -x2 : 0.0;
-}
-
 // one CTA per (pair, K): the information matrix of every trial budget's best model, from usip_ransac_rt_f64's
 // best_trial / status; dynamic smem: the points and match list of ransac_kernel, and the inlier flags
 __global__ void __launch_bounds__(REG_THREADS)
@@ -589,10 +596,7 @@ ransac_info_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ co
       for (int m = 0; m < npts; ++m) {
         if (!flag[m]) continue;
         const int a = mi[m] & 0xffff;
-        double ar[3], ac[3];
-        reg_info_col(r, ax[a], ay[a], az[a], ar);
-        reg_info_col(c, ax[a], ay[a], az[a], ac);
-        s = __dadd_rn(s, __dadd_rn(__dadd_rn(__dmul_rn(ar[0], ac[0]), __dmul_rn(ar[1], ac[1])), __dmul_rn(ar[2], ac[2])));
+        s = __dadd_rn(s, reg_info_entry(r, c, ax[a], ay[a], az[a]));
         ++n;
       }
       info_out[o * 36 + tid] = s;
@@ -635,11 +639,26 @@ extern "C" int usip_desc_match_f64(const float* desc, const int32_t* count, int 
   if (int e = reg_check_ks(ks, nK, kk)) return e;
   const int cap = k == 1 ? L : 2 * k * L;
   const int smem = k == 1 ? 0 : (L * ((L + 31) / 32) + L + 1) * (int)sizeof(uint32_t);
-  cudaError_t e = cudaFuncSetAttribute(desc_match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  cudaError_t e = cudaFuncSetAttribute(desc_match_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) { set_last_error("desc_match: smem attribute"); return (int)e; }
-  desc_match_kernel<<<P * nK, REG_THREADS, smem, (cudaStream_t)stream>>>(desc, count, L, D, pairs, kk, nK, k, cap,
-                                                                         matches, n_matches);
+  desc_match_kernel<false><<<P * nK, REG_THREADS, smem, (cudaStream_t)stream>>>(desc, count, L, D, pairs, kk, nK, k,
+                                                                                cap, matches, n_matches);
   return check_launch("desc_match_kernel");
+}
+
+extern "C" int usip_desc_match_mutual_f64(const float* desc, const int32_t* count, int n_scans, int L, int D,
+                                          const int32_t* pairs, int P, const int32_t* ks, int nK, int32_t* matches,
+                                          int32_t* n_matches, void* stream) {
+  USIP_REQUIRE(desc && count && pairs && matches && n_matches, "desc_match_mutual: null pointer");
+  USIP_REQUIRE(n_scans > 0 && L > 0 && D > 0 && P > 0, "desc_match_mutual: bad sizes");
+  USIP_REQUIRE(D <= USIP_REG_MAX_DIM, "desc_match_mutual: descriptor length over USIP_REG_MAX_DIM");
+  USIP_REQUIRE(L <= USIP_REG_MAX_KEYPOINTS, "desc_match_mutual: more keypoints per scan than shared memory holds");
+  RegKs kk;
+  if (int e = reg_check_ks(ks, nK, kk)) return e;
+  const int smem = 2 * L * (int)sizeof(int32_t);
+  desc_match_kernel<true><<<P * nK, REG_THREADS, smem, (cudaStream_t)stream>>>(desc, count, L, D, pairs, kk, nK, 1, L,
+                                                                               matches, n_matches);
+  return check_launch("desc_match_kernel<mutual>");
 }
 
 extern "C" int usip_ransac_rt_f64(const float* xyz, const int32_t* count, int n_scans, int L, const int32_t* pairs,

@@ -8,6 +8,8 @@ sweep and every maxTrials of a sweep at once.
     res = ev.score()
     print("\\n".join(res.lines()))
     ev.write_registration_logs(out_dir, K=512, max_trials=30000)
+    res = ev.score(solver="fgr")                   # Fast Global Registration instead of RANSAC
+    ev.write_registration_logs(out_dir, K=512)
 
 Per scene, the fragment pairs are every i < j by frame number (pairs="all", runFragmentRegistration.m) or the gt.log
 pairs only (pairs="gt", the overlapped-pairs variant).  Frames are the identity.  Per pair and K, on the device:
@@ -30,6 +32,21 @@ Deliberate deviations from the reference:
   * The .log is written straight from the kernels' fp64 results (%.10f), not re-read from the %15.8e of a per-pair
     .rt.txt.
   * 3DMatch fragments are taken in frame order (indoor_test_loader.py).
+
+solver="fgr" registers with Fast Global Registration instead (evaluation/matlab/eval_indoor/fgr/,
+register2FragmentsFGR.m; usip_desc_match_mutual_f64 and usip_fgr_f64, see include/usip_b200.h): mutual nearest
+descriptor matches, FGR's tuple test and its 640 graduated non-convexity iterations, for every pair and K in one launch.
+The trial axis then has length 1 and no maxTrials.  Its further deviations:
+  * register2FragmentsFGR.m writes constant statistics (numInliers 1, inlierRatio 0.99, ratioAligned 0.8) and no
+    information matrix.  Here they are measured under the final T: the mutual matches within 0.2 (the RANSAC inlier
+    test), inlierRatio = inliers / mutual matches, info = sum A^T A over them as for RANSAC, and the overlap test and
+    writeLog.m's filters run as for RANSAC (overlap_threshold None keeps ratioAligned = 0.8).
+  * The library seeds rand() with time(NULL); here the tuple draws are Philox4x32-10 keyed by the seed, the same stream
+    for every pair and K.
+  * The library matches with FLANN and moves the points in float; here everything is fp64.
+  * The library divides by zero with no correspondences; here that, like any pair with fewer than 10 tuple
+    correspondences, gets no iterations (status 1).  A fragment whose centred points all coincide (scale 0) is status
+    4.  Only status 0 counts as a model, as for RANSAC.
 
 Descriptors (describe, with a ModelDescriptorIndoor): DescriptorLiteOldGlobal's global context is the max over the
 keypoints the descriptor is given.  describe() gives it all M keypoints of the detector pass, before NMS and before the
@@ -61,6 +78,9 @@ DEFAULT_OVERLAP_THRESHOLD = 0.23          # writeLog.m: resultAlignRatio(1) > 0.
 INLIER_RATIO_THRESHOLD = 0.025            # writeLog.m: resultInlierRatio > 0.025
 ERR2 = 0.04                               # mrEvaluateRegistrationMy.m
 MATCH_BUFFER_BYTES = 1 << 28              # pairs per launch: the match list of one chunk stays under 256 MB
+SOLVERS = ("ransac", "fgr")
+FGR_MAX_DIM = 512                         # USIP_REG_MAX_DIM
+FGR_MAX_ROWS = 1024                       # USIP_REG_MAX_KEYPOINTS
 
 
 # ----------------------------------------------------------------------------------------------- files
@@ -238,14 +258,51 @@ def score_logs(log_dir, scenes, eval_dir):
     return out, line, means
 
 
+# ----------------------------------------------------------------------------------------------- one pair
+def _rows(a, cols, what):
+    t = torch.as_tensor(a) if not isinstance(a, torch.Tensor) else a
+    t = t.detach().to(torch.float32)
+    if t.dim() != 2 or (cols is not None and t.shape[1] != cols):
+        raise ValueError("%s must be (n, %s)" % (what, cols if cols is not None else "D"))
+    return t
+
+
+def fast_global_registration(points1, features1, points2, features2, seed=0):
+    """fast_global_registration.cpp's interface for one pair: points (n_f, 3) and features (n_f, D), numpy or CUDA
+    tensors, at most 1024 rows and 512 dims -> T (4, 4) float64 with T[:3, :3] points2 + T[:3, 3] aligned to points1.
+    Runs usip_desc_match_mutual_f64 and usip_fgr_f64 on the pair; with fewer than 10 tuple correspondences (or a
+    degenerate scale) T is [I | mean1 - mean2], as the mex returns."""
+    p1, p2 = _rows(points1, 3, "points1"), _rows(points2, 3, "points2")
+    f1, f2 = _rows(features1, None, "features1"), _rows(features2, None, "features2")
+    if len(f1) != len(p1) or len(f2) != len(p2) or f1.shape[1] != f2.shape[1]:
+        raise ValueError("features must have one row per point and the same length on both sides")
+    n1, n2, D = len(p1), len(p2), f1.shape[1]
+    if not 1 <= D <= FGR_MAX_DIM or max(n1, n2) > FGR_MAX_ROWS:
+        raise ValueError("at most %d rows and 1 to %d feature dims" % (FGR_MAX_ROWS, FGR_MAX_DIM))
+    dev = next((t.device for t in (p1, p2, f1, f2) if t.is_cuda), torch.device("cuda"))
+    L = max(n1, n2, 1)
+    xyz = torch.zeros((2, L, 3), dtype=torch.float32, device=dev)
+    desc = torch.zeros((2, L, D), dtype=torch.float32, device=dev)
+    xyz[0, :n1], xyz[1, :n2] = p1.to(dev), p2.to(dev)
+    desc[0, :n1], desc[1, :n2] = f1.to(dev), f2.to(dev)
+    count = torch.tensor([n1, n2], dtype=torch.int32, device=dev)
+    pairs = torch.tensor([[0, 1]], dtype=torch.int32, device=dev)
+    m, n = ops.desc_match_mutual(desc, count, pairs, [L])
+    out = ops.fgr(xyz, count, pairs, [L], m, n, INLIER_THRESHOLD, seed)
+    T = np.eye(4)
+    T[:3] = out["Rt"][0, 0].cpu().numpy()
+    return T
+
+
 # ----------------------------------------------------------------------------------------------- the evaluator
 class IndoorRegistrationResult:
     """Per scene: pairs (P, 2) frame numbers, n_fragments, n_matches (P, nK), and per (pair, K, maxTrials) arrays Rt
     (.., 4, 4) (the identity without a model), n_inliers, inlier_ratio, aligned (ratioAligned(1), NaN where not
     computed), info (.., 6, 6) and accepted (the log's filter).  scores[(K, maxTrials)] = ({scene: evaluate dict},
-    summary line, means)."""
+    summary line, means).  solver "fgr": one trial entry, maxTrials None."""
 
-    def __init__(self, dataset, keypoint_nums, max_trials, overlap_threshold, scenes, per_scene, gt):
+    def __init__(self, dataset, keypoint_nums, max_trials, overlap_threshold, scenes, per_scene, gt, solver="ransac"):
+        self.solver = solver
         self.dataset, self.keypoint_nums, self.max_trials = dataset, list(keypoint_nums), list(max_trials)
         self.overlap_threshold, self.scenes, self.per_scene = overlap_threshold, list(scenes), per_scene
         self.scores = {}
@@ -266,9 +323,11 @@ class IndoorRegistrationResult:
     def lines(self):
         out = []
         for (K, T), (sc, line, _) in self.scores.items():
+            head = "K=%d FGR %s" % (K, self.dataset) if self.solver == "fgr" else \
+                "K=%d maxTrials=%d %s" % (K, T, self.dataset)
             for s in self.scenes:
-                out += ["K=%d maxTrials=%d %s: %s" % (K, T, self.dataset, v) for v in scene_lines(s, sc[s])]
-            out.append("K=%d maxTrials=%d %s: %s" % (K, T, self.dataset, line))
+                out += ["%s: %s" % (head, v) for v in scene_lines(s, sc[s])]
+            out.append("%s: %s" % (head, line))
         return out
 
     def to_dict(self):
@@ -280,7 +339,8 @@ class IndoorRegistrationResult:
                          "log_entries": {s: int(self.per_scene[s]["accepted"][:, self.keypoint_nums.index(K),
                                                                                  self.max_trials.index(T)].sum())
                                          for s in self.scenes}})
-        return {"dataset": self.dataset, "keypoint_nums": self.keypoint_nums, "max_trials": self.max_trials,
+        return {"dataset": self.dataset, "solver": self.solver, "keypoint_nums": self.keypoint_nums,
+                "max_trials": None if self.solver == "fgr" else self.max_trials,
                 "overlap_threshold": self.overlap_threshold,
                 "pairs": {s: int(len(self.per_scene[s]["pairs"])) for s in self.scenes}, "runs": runs}
 
@@ -347,20 +407,30 @@ class IndoorRegistration(Registration):
         offsets = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int64)
         return torch.from_numpy(np.concatenate(rows)).to(src.device), offsets, where
 
-    def _register(self, scene, fp, ks, ts, seed, uniforms):
-        """Matching, RANSAC and the information matrix of one scene's pairs fp (P, 2 frames), a chunk of pairs per launch
-        -> dict of numpy arrays."""
+    def _register(self, scene, fp, ks, ts, seed, uniforms, solver="ransac"):
+        """Matching, then RANSAC and the information matrix (solver "ransac") or mutual matching and FGR (solver "fgr",
+        one trial entry), of one scene's pairs fp (P, 2 frames), a chunk of pairs per launch -> dict of numpy arrays."""
         dev = self.xyz.device
         L = min(self.xyz.shape[1], ks[-1])
         xyz, desc = self.xyz[:, :L].contiguous(), self.desc[:, :L].contiguous()
         count = torch.clamp(self.count, max=L).to(torch.int32).contiguous()
-        chunk = max(1, MATCH_BUFFER_BYTES // (len(ks) * 2 * MATCH_K * L * 8))
+        per_pair = len(ks) * L * 8 if solver == "fgr" else len(ks) * 2 * MATCH_K * L * 8
+        chunk = max(1, MATCH_BUFFER_BYTES // per_pair)
         keys = ("n_matches", "Rt", "n_inliers", "status", "info", "n_info")
         parts = {k: [] for k in keys}
         for c0 in range(0, len(fp), chunk):
             sel = fp[c0:c0 + chunk]
             pairs = torch.tensor([[self.index[(scene, int(a))], self.index[(scene, int(b))]] for a, b in sel],
                                  dtype=torch.int32, device=dev).reshape(-1, 2)
+            if solver == "fgr":
+                m, n = ops.desc_match_mutual(desc, count, pairs, ks)
+                out = ops.fgr(xyz, count, pairs, ks, m, n, INLIER_THRESHOLD, seed)
+                got = {"n_matches": n, "Rt": out["Rt"][:, :, None], "n_inliers": out["n_inliers"][:, :, None],
+                       "status": out["status"][:, :, None], "info": out["info"][:, :, None],
+                       "n_info": out["n_inliers"][:, :, None]}
+                for k in keys:
+                    parts[k].append(got[k].cpu().numpy())
+                continue
             frames = torch.from_numpy(np.broadcast_to(np.eye(3, 4), (len(sel), 3, 3, 4)).copy()).to(dev)
             m, n = ops.desc_match(desc, count, pairs, ks, MATCH_K)
             out = ops.ransac_rt(xyz, count, pairs, frames, m, n, ts, INLIER_THRESHOLD, seed, uniforms)
@@ -372,13 +442,21 @@ class IndoorRegistration(Registration):
                 parts[k].append(got[k].cpu().numpy())
         return {k: np.concatenate(v) for k, v in parts.items()}
 
-    def score(self, keypoint_nums=DEFAULT_KEYPOINT_NUMS, max_trials=DEFAULT_MAX_TRIALS,
-              overlap_threshold=DEFAULT_OVERLAP_THRESHOLD, pairs="all", seed=0, uniforms=None):
-        """Registers every pair of every scene for every K and maxTrials, runs the overlap test where it can decide the
-        log, filters and scores -> IndoorRegistrationResult (also kept as self.result).  overlap_threshold None skips
-        the overlap test (the lite variant's ratioAligned = 0.8)."""
+    def score(self, keypoint_nums=DEFAULT_KEYPOINT_NUMS, max_trials=None,
+              overlap_threshold=DEFAULT_OVERLAP_THRESHOLD, pairs="all", seed=0, uniforms=None, solver="ransac"):
+        """Registers every pair of every scene for every K and maxTrials (DEFAULT_MAX_TRIALS when None), runs the overlap
+        test where it can decide the log, filters and scores -> IndoorRegistrationResult (also kept as self.result).
+        overlap_threshold None skips the overlap test (the lite variant's ratioAligned = 0.8).  solver "fgr" registers
+        with Fast Global Registration: no maxTrials and no uniforms, one trial entry."""
+        if solver not in SOLVERS:
+            raise ValueError("solver must be 'ransac' or 'fgr', got %r" % (solver,))
         ks = check_sweep(keypoint_nums, 1.0)
-        ts = check_trials(max_trials, INLIER_THRESHOLD)
+        if solver == "fgr":
+            if max_trials is not None or uniforms is not None:
+                raise ValueError("solver 'fgr' takes no max_trials and no uniforms")
+            ts = [None]
+        else:
+            ts = check_trials(DEFAULT_MAX_TRIALS if max_trials is None else max_trials, INLIER_THRESHOLD)
         _check_keypoint_limit(ks)
         if self.xyz is None:
             raise RuntimeError("describe() or read_descriptor_tree() first")
@@ -389,10 +467,10 @@ class IndoorRegistration(Registration):
         per_scene = {}
         for scene in self.scenes:
             fp = self.scene_pairs(scene, pairs)
-            r = self._register(scene, fp, ks, ts, seed, uniforms) if len(fp) else None
+            r = self._register(scene, fp, ks, ts, seed, uniforms, solver) if len(fp) else None
             per_scene[scene] = self._finish(scene, fp, r, len(ks), len(ts), overlap_threshold)
         self.result = IndoorRegistrationResult(self.dataset, ks, ts, overlap_threshold, self.scenes, per_scene,
-                                               self.gt)
+                                               self.gt, solver)
         return self.result
 
     def _finish(self, scene, fp, r, nK, nT, overlap_threshold):
@@ -436,12 +514,16 @@ class IndoorRegistration(Registration):
         rows = np.diff(offsets)
         return np.array([hits[s] / rows[jobs[s][0]] for s in of], dtype=np.float64)
 
-    def write_registration_logs(self, out_dir, K, max_trials):
-        """writeLog.m for the last score's K and maxTrials: <out_dir>/<scene>.log, one entry per accepted pair."""
+    def write_registration_logs(self, out_dir, K, max_trials=None):
+        """writeLog.m for the last score's K and maxTrials (None for an FGR score): <out_dir>/<scene>.log, one entry per
+        accepted pair."""
         if self.result is None:
             raise RuntimeError("score() first")
         res = self.result
-        k, t = res.keypoint_nums.index(int(K)), res.max_trials.index(int(max_trials))
+        if (res.solver == "fgr") != (max_trials is None):
+            raise ValueError("max_trials is None exactly for an FGR score")
+        k = res.keypoint_nums.index(int(K))
+        t = 0 if max_trials is None else res.max_trials.index(int(max_trials))
         os.makedirs(out_dir, exist_ok=True)
         for scene in self.scenes:
             e = res.log_entries(scene, k, t)
@@ -476,7 +558,10 @@ def main(argv=None):
     ap.add_argument("--feature-dim", type=int, default=128, help="descriptor length of --descriptor-tree")
     ap.add_argument("--pairs", choices=("all", "gt"), default="all")
     ap.add_argument("--keypoint-nums", type=int, nargs="+", default=list(DEFAULT_KEYPOINT_NUMS))
-    ap.add_argument("--max-trials", type=int, nargs="+", default=list(DEFAULT_MAX_TRIALS))
+    ap.add_argument("--solver", choices=SOLVERS, default="ransac",
+                    help="ransac (register2Fragments.m) or fgr (register2FragmentsFGR.m, Fast Global Registration)")
+    ap.add_argument("--max-trials", type=int, nargs="+", help="RANSAC trial budgets (default %s)"
+                    % " ".join(str(t) for t in DEFAULT_MAX_TRIALS))
     ap.add_argument("--overlap-threshold", default=str(DEFAULT_OVERLAP_THRESHOLD),
                     help="writeLog.m's ratioAligned(1) threshold, or 'none' to skip the overlap test")
     ap.add_argument("--write-logs", metavar="DIR", help="write <DIR>/<scene>.log for the largest K and maxTrials")
@@ -491,6 +576,10 @@ def main(argv=None):
     a = ap.parse_args(argv)
     if a.dataset == "redwood" and not a.gt_root:
         ap.error("redwood needs --gt-root")
+    if a.solver == "fgr" and a.max_trials is not None:
+        ap.error("--max-trials applies to --solver ransac only")
+    if a.solver == "ransac" and a.max_trials is None:
+        a.max_trials = list(DEFAULT_MAX_TRIALS)
     if a.score_logs:
         scenes = [s for s, _ in REDWOOD_SCENES] if a.dataset == "redwood" else list(MATCH3D_SCENES)
         sc, line, means = score_logs(a.score_logs, scenes, _scene_eval_dir(a.dataset, a.root, a.gt_root))
@@ -505,7 +594,8 @@ def main(argv=None):
     thr = None if a.overlap_threshold.lower() == "none" else float(a.overlap_threshold)
     ks = check_sweep(a.keypoint_nums, 1.0)
     _check_keypoint_limit(ks)
-    check_trials(a.max_trials, INLIER_THRESHOLD)
+    if a.solver == "ransac":
+        check_trials(a.max_trials, INLIER_THRESHOLD)
     if not a.root:
         ap.error("give --root")
     hc = detector_from_args(a, ap)
@@ -532,12 +622,13 @@ def main(argv=None):
             load_detector_checkpoint(det, a.detector)
         load_descriptor_checkpoint(des, a.descriptor)
         ev.describe(det, des, a.nms_radius, L=ks[-1])
-    res = ev.score(ks, a.max_trials, thr, a.pairs, a.seed)
+    extra = () if a.solver == "ransac" else (None, a.solver)            # (uniforms, solver)
+    res = ev.score(ks, a.max_trials, thr, a.pairs, a.seed, *extra)
     print("\n".join(res.lines()))
     if hc is not None and not a.descriptor_tree:
         print(hc.count_summary())
     if a.write_logs:
-        ev.write_registration_logs(a.write_logs, ks[-1], a.max_trials[-1])
+        ev.write_registration_logs(a.write_logs, ks[-1], a.max_trials[-1] if a.solver == "ransac" else None)
     if a.json:
         with open(a.json, "w") as f:
             json.dump(res.to_dict(), f, indent=1)

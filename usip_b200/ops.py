@@ -475,6 +475,50 @@ def ransac_info(xyz, count, pairs, frames, matches, n_matches, trials, best_tria
     return info, n_info
 
 
+def desc_match_mutual(desc, count, pairs, ks):
+    """Mutual nearest-neighbour matches (FGR's AdvancedMatching cross-check) for every pair and K at once
+    (include/usip_b200.h usip_desc_match_mutual_f64).  desc (S,L,D) f32, count (S,) i32, pairs (P,2) i32, all CUDA; ks
+    ascending ints (host) -> (matches (P,nK,L,2) i32, n_matches (P,nK) i32), ascending by anchor row."""
+    _req(desc, f32, "desc"); _req(count, i32, "count"); _req(pairs, i32, "pairs")
+    S, L, D = desc.shape
+    P = pairs.shape[0]
+    if tuple(count.shape) != (S,) or pairs.dim() != 2 or pairs.shape[1] != 2:
+        raise ValueError("count must be (%d,) and pairs (P, 2)" % S)
+    ks_h = (ctypes.c_int32 * len(ks))(*[int(v) for v in ks])
+    matches = torch.empty((P, len(ks), L, 2), dtype=i32, device=desc.device)
+    n = torch.empty((P, len(ks)), dtype=i32, device=desc.device)
+    with torch.cuda.device(desc.device):
+        check(_lib.load().usip_desc_match_mutual_f64(_p(desc), _p(count), S, L, D, _p(pairs), P, ks_h, len(ks),
+                                                     _p(matches), _p(n), _stream()), "usip_desc_match_mutual_f64")
+    return matches, n
+
+
+def fgr(xyz, count, pairs, ks, matches, n_matches, threshold=0.2, seed=0):
+    """Fast Global Registration of every pair and K at once (include/usip_b200.h usip_fgr_f64).  xyz (S,L,3) f32, count
+    (S,) i32, pairs (P,2) i32, matches / n_matches from desc_match_mutual, all CUDA; ks the same ascending ints (host):
+    fragment f of a (pair, K) is its scan's first min(K, count, L) rows -> dict of Rt (P,nK,3,4) f64, n_tuples,
+    n_inliers, status (P,nK) i32 and info (P,nK,6,6) f64."""
+    _req(xyz, f32, "xyz"); _req(count, i32, "count"); _req(pairs, i32, "pairs")
+    _req(matches, i32, "matches"); _req(n_matches, i32, "n_matches")
+    S, L, _ = xyz.shape
+    P, nK, cap = matches.shape[0], matches.shape[1], matches.shape[2]
+    if tuple(xyz.shape) != (S, L, 3) or tuple(count.shape) != (S,) or tuple(pairs.shape) != (P, 2):
+        raise ValueError("xyz must be (S, L, 3), count (S,) and pairs (P, 2)")
+    if tuple(matches.shape) != (P, nK, cap, 2) or tuple(n_matches.shape) != (P, nK) or len(ks) != nK:
+        raise ValueError("matches must be (P, nK, cap, 2) and n_matches (P, nK), nK = len(ks)")
+    ks_h = (ctypes.c_int32 * nK)(*[int(v) for v in ks])
+    dev = xyz.device
+    e = lambda: torch.empty((P, nK), dtype=i32, device=dev)
+    out = {"Rt": torch.empty((P, nK, 3, 4), dtype=torch.float64, device=dev), "n_tuples": e(), "n_inliers": e(),
+           "info": torch.empty((P, nK, 6, 6), dtype=torch.float64, device=dev), "status": e()}
+    with torch.cuda.device(dev):
+        check(_lib.load().usip_fgr_f64(
+            _p(xyz), _p(count), S, L, _p(pairs), P, ks_h, nK, _p(matches), _p(n_matches), cap,
+            int(seed) & (2 ** 64 - 1), float(threshold), _p(out["Rt"]), _p(out["n_tuples"]), _p(out["n_inliers"]),
+            _p(out["info"]), _p(out["status"]), _stream()), "usip_fgr_f64")
+    return out
+
+
 def fragment_overlap(xyz, offsets, jobs, Rt, radius=0.2):
     """register2Fragments.m's aligned-point count (include/usip_b200.h usip_fragment_overlap_f32): xyz (R,3) f32 CUDA,
     every fragment's rows packed; offsets (n_frags + 1,) ints and jobs (J, 2) ints (fragment a, fragment b), host
